@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — CTR training samples/s of DeepFM on a synthetic Criteo-shaped batch (BASELINE.json).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one pass of the hot path over one batch: clear_grad -> DeepFMLayer.forward (fused
@@ -10,18 +10,23 @@ grad) -> optimizer step (lazy Adam on the touched rows, Adam on the dense parame
 
 Workload (config.workload): DeepFM, 26 sparse + 13 dense slots, hashed vocab V=1e8, D=16,
 B=65536 per GPU, fc [400,400,400], uniform hashed ids with 2 % padding, 8 rotating batches
-(per-step working set: 164 MB feat + 6.4 GB table >> 126 MB L2, so no L2 flush is needed).
+(per-step working set: 164 MB feat + 6.4 GB table >> 50 MB L2, so no L2 flush is needed).
 N>1: tables row-sharded (owner = id mod N), NCCL all-to-all of ids/rows/grads, dense grads
 all-reduced; weak scaling (B per GPU fixed).
 
-Printed JSON (one line, rank 0): see the contract in the task statement; extra keys `roofline`
-(fused gather+FM forward kernel, algorithmic bytes / CUDA-event time inside the timed region
-against MEASURED_PEAKS.json), `cpu_baseline` (oracle port timed on the host cores, N=1 only),
+Printed JSON (one line, rank 0): metric, value, unit, steps, ms_per_step, config; extra keys
+`roofline` (fused gather+FM forward kernel, algorithmic bytes / CUDA-event time inside the timed
+region against MEASURED_PEAKS.json when present, else the H100 SXM data sheet), `cpu_baseline` (oracle port timed on the host cores, N=1 only),
 `e2e` (same metric through the public API — runner.DevicePrefetcher over pinned HOST batches +
 DygraphModel.train_forward incl. its AUC update: H2D of every batch and D2H of the loss inside the
 timed region), `roofline_step` (CUDA-event time of every kernel family of the step + the
 composite bound of the whole step), `clocks`, `gpu_launches`; at N>1 also `parity` (step-0 loss
 of the sharded model == the fp64 oracle on a slice of the global batch).
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed as float32 .npy
+files (rank 0): pred [B, 1] and loss of that step, every dense parameter after its optimizer step,
+and the table rows of a fixed seeded sample of 4096 ids of that step's batch (the whole table is GBs).
+The inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -60,6 +65,8 @@ def parse():
     p.add_argument("--no-cpu-baseline", action="store_true")
     p.add_argument("--timeline", default="", help="write a CUPTI timeline of 3 steps (rank 0) "
                    "as <path>.json (chrome trace) and <path>.txt (per-stream summary) and exit")
+    p.add_argument("--dump-outputs", default="", metavar="DIR",
+                   help="write what the last timed step computed to DIR/<name>.npy (float32)")
     return p.parse_args()
 
 
@@ -88,7 +95,7 @@ def make_batches(n, B, V, dist, seed, pin):
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -134,7 +141,7 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 # -------------------------------------------------------------------------------- reference arm
@@ -213,7 +220,8 @@ def workload_config(args, world):
             "parallelism": "single GPU" if world == 1 else
             "tables row-sharded (id mod %d) + %s; dense params data-parallel (NCCL all-reduce)" %
             (world, exchange_name(world)),
-            "l2": "inputs larger than L2 (8 rotating batches; 164 MB feat + 6.4 GB table per step)"}
+            "l2": "inputs larger than the 50 MB L2 (8 rotating batches; 164 MB feat + 6.4 GB table "
+                  "per step)"}
 
 
 # ------------------------------------------------------------------------------------- our arm
@@ -259,6 +267,8 @@ def run_b200(args, rank, world, local_rank):
     prefetch = getattr(model, "prefetch", None)
     finish_prefetch = getattr(model, "finish_prefetch", None)
 
+    last = {}
+
     def step_resident(i):
         label, ids, dense = resident[i % len(resident)]
         optimizer.clear_grad()
@@ -270,6 +280,7 @@ def run_b200(args, rank, world, local_rank):
         if finish_prefetch is not None:
             finish_prefetch()
         optimizer.step()
+        last.update(pred=pred, loss=loss, ids=ids)
         return loss
 
     from paddlerec_b200 import runner
@@ -338,6 +349,8 @@ def run_b200(args, rank, world, local_rank):
     parity = parity_bit(args, model, dm, resident, label_f, rank, world, dev) if world > 1 else None
     ms, launches, events, clocks = timed(step_resident, K, W, collect_events=True,
                                          event_filter={"embed_fm_fwd"})
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, model, last, rank, world)
     value = args.batch * world * K / (ms / 1e3)
     k_ms = [s.elapsed_time(e) for (name, s, e) in events if name == "embed_fm_fwd"]
     kernel_ms = sum(k_ms) / max(len(k_ms), 1)
@@ -354,12 +367,6 @@ def run_b200(args, rank, world, local_rank):
     if rank != 0:
         return
     peak, peak_src = measured_peaks()
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "k1_traffic.json")
-    if os.path.exists(tpath) and args.dim == 16 and args.batch == 65536:
-        with open(tpath) as fh:
-            t = json.load(fh)
-        traffic = t["dram_bytes_read_per_launch"] + t["dram_bytes_write_per_launch"]
     alg = algorithmic_bytes_fwd(args.dim) * args.batch
     achieved = alg / (kernel_ms / 1e3) / 1e9 if kernel_ms > 0 else 0.0
     line = {
@@ -374,9 +381,7 @@ def run_b200(args, rank, world, local_rank):
                      "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                      "frac": achieved / peak, "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": alg, "kernel_ms": kernel_ms,
-                     "kernel_share_of_step": kernel_ms / (ms / K), "traffic": traffic,
-                     "traffic_source": "profiles/k1_traffic.json (ncu --set full, one launch)",
-                     "frac_of_nominal_8TBs": achieved / 8000.0},
+                     "kernel_share_of_step": kernel_ms / (ms / K)},
         "e2e": {"value": e2e_value, "unit": "samples/s", "ms_per_step": ms_e2e / K,
                 "h2d_bytes_per_step": args.batch * (F_SPARSE * 8 + N_DENSE * 4 + 8),
                 "d2h_bytes_per_step": 4},
@@ -391,6 +396,29 @@ def run_b200(args, rank, world, local_rank):
         except Exception as exc:  # the GPU numbers stand on their own
             line["cpu_baseline"] = {"error": repr(exc)}
     print(json.dumps(line), flush=True)
+
+
+def dump_outputs(path, model, last, rank, world):
+    """What the last timed step computed, as float32 .npy files (see the module docstring)."""
+    import numpy as np
+
+    torch.cuda.synchronize()
+    if rank != 0:
+        return
+    os.makedirs(path, exist_ok=True)
+    out = {"pred": last["pred"], "loss": last["loss"].reshape(1)}
+    flat = last["ids"].reshape(-1)
+    g = torch.Generator().manual_seed(20240601)
+    ids = flat[torch.randint(0, flat.numel(), (4096,), generator=g).to(flat.device)]
+    if world > 1:                     # rows this rank owns (owner = id mod N, local row = id div N)
+        ids = ids[ids % world == rank] // world
+    for name, p in model.named_parameters():
+        if p.numel() > (4 << 20):     # an embedding table: the sampled rows only
+            out["rows." + name] = p.detach()[ids]
+        else:
+            out["param." + name] = p.detach()
+    for name, t in out.items():
+        np.save(os.path.join(path, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 def timeline(path, step, barrier, rank, warmup):
@@ -474,8 +502,9 @@ def roofline_step(args, per_ms, step_ms, step_ms_with_events, world):
     if os.path.exists(path):
         with open(path) as fh:
             peaks = json.load(fh)
-    tf = float(peaks.get("bf16_tflops_sustained", 1400.0))
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
+    # without MEASURED_PEAKS.json: the H100 SXM data sheet (dense BF16, HBM3), not a sustained rate
+    tf = float(peaks.get("bf16_tflops_sustained", 989.0))
+    hbm = float(peaks.get("hbm_gbs", 3350.0))
     G = (D + 1 + 3) // 4 * 4
     k1 = algorithmic_bytes_fwd(D) * B
     k2 = (F * 8 + (F + Dn) * 4 * D + F * 4 * D + F * 2 * 4 * D) * B
@@ -495,7 +524,7 @@ def roofline_step(args, per_ms, step_ms, step_ms_with_events, world):
                        "achieved_tflops": round(flops / (gemm_ms / 1e3) / 1e12, 1) if gemm_ms else None,
                        "peak_tflops_sustained": tf,
                        "frac": round(flops / (gemm_ms / 1e3) / 1e12 / tf, 3) if gemm_ms else None,
-                       "kernels": "tc_gemm_kmajor_kernel / tc_gemm_dw_kernel (tcgen05 + TMEM + TMA)"},
+                       "kernels": "tc_gemm_kmajor_kernel / tc_gemm_dw_kernel (wgmma + TMA)"},
         "composite_bound": {"gemm_ms": round(flops / (tf * 1e12) * 1e3, 4),
                             "hbm_ms": round(hbm_bytes / (hbm * 1e9) * 1e3, 4),
                             "hbm_bytes": int(hbm_bytes), "bound_ms": round(bound_ms, 4),

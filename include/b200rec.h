@@ -1,5 +1,5 @@
 /*
- * b200rec.h — C ABI of the B200-native sparse-embedding + feature-interaction engine.
+ * b200rec.h — C ABI of the H100-native sparse-embedding + feature-interaction engine.
  *
  * This is the drop-in boundary for the one hot path of PaddleRec's rank models
  * (reference checkout /root/reference, commit 656326ad):
@@ -65,10 +65,10 @@ int b200rec_oob_count(uint64_t* count_host, int reset, void* stream);
  * feat:[B,F+Dn,D]  y1,y2:[B]  S:[B,D] (saved for backward; may be NULL).
  * padding_idx < 0 means "no padding row".  D must be <=128 (D%4==0), <=64 (D%2==0) or <=32.
  * Row strides (in floats): row i of the second-order table starts at W + i*ldw, its first-order
- * weight is W1[i*ldw1].  Two separate tables: ldw=D, ldw1=1.  The B200-native FUSED layout keeps
+ * weight is W1[i*ldw1].  Two separate tables: ldw=D, ldw1=1.  The FUSED layout keeps
  * both in one 128-byte slot [D emb | w1 | pad] (ldw = ldw1 = 32, W1 = W + D): a random 64-byte
- * row and a random 4-byte scalar each cost a full 128-byte DRAM access on this part
- * (profiles/r1_gather_variants_microbench.txt), so the slot halves the random traffic. */
+ * row and a random 4-byte scalar each cost a full 128-byte DRAM access
+ * (tools/microbench/gather_variants.cu measures it), so the slot halves the random traffic. */
 int b200rec_embed_fm_fwd(const float* W, int64_t ldw, const float* W1, int64_t ldw1,
                          const int64_t* ids, const float* dense, const float* dense_w,
                          const float* dense_w1, float* feat, float* y1, float* y2, float* S,
@@ -229,8 +229,8 @@ int b200rec_tower_prep_weight(const float* W, void* W2r_bf16, void* W2c_bf16, vo
                               int K, int N, void* stream);
 int b200rec_tower_fold_dw(const float* Mx, float* dW, int K, int N, void* stream);
 
-/* ---- tower GEMMs on the 5th-gen tensor cores (csrc/tc_gemm.cuh) ----------- */
-/* Hand-written tcgen05.mma / TMEM / TMA kernels that replace the library GEMMs of the dense tower
+/* ---- tower GEMMs on the Hopper tensor cores (csrc/tc_gemm.cuh) ------------ */
+/* Hand-written wgmma / TMA kernels that replace the library GEMMs of the dense tower
  * (DNN.forward, models/rank/deepfm/net.py:169-174; dcn_v2/net.py:178-184; CrossNetV2
  * dcn_v2/net.py:222-226) and of its backward (tools/trainer.py:151).  fp32 products are evaluated
  * as a_hi*b_hi + a_lo*b_hi + a_hi*b_lo on bf16 operands with fp32 accumulation ("bf16x3").
@@ -310,9 +310,7 @@ int b200rec_log_loss_mean_bwd(const float* pred, const void* label, int label_is
 int b200rec_auc_update(const float* pred, const void* label, int label_is_i64, int64_t* stat_pos,
                        int64_t* stat_neg, int num_thresholds, int64_t n, void* stream);
 /* tuning / bring-up knobs (key 0: force tile width BN; 1-3: descriptor overrides of the dW kernel;
- * 4: k-block of the K-major kernel, 64 = 128-byte swizzle, 32 = 64-byte swizzle, more stages;
- * 5: epilogue outputs through TMA bulk stores (1) or register stores (0); 6: K-major GEMM on CTA
- * pairs (tcgen05 cta_group::2, 256-row tiles) for M >= 4096)
+ * 4: k-block of the K-major kernel, 64 = 128-byte swizzle, 32 = 64-byte swizzle, more stages)
  * and the device word a pipeline watchdog writes before it traps. */
 int b200rec_tc_debug(int key, int value);
 int b200rec_tc_timeout_word(unsigned int* word_host);

@@ -1,7 +1,7 @@
-"""paddlerec_b200 — B200-native sparse-embedding + feature-interaction engine behind PaddleRec's
+"""paddlerec_b200 — H100-native sparse-embedding + feature-interaction engine behind PaddleRec's
 rank-model surface (models/rank/*/net.py, DygraphModel).  See DESIGN.md.
 
-  csrc/            hand-written sm_100a CUDA kernels + the C ABI (include/b200rec.h)
+  csrc/            hand-written sm_90a CUDA kernels + the C ABI (include/b200rec.h)
   _lib.py          ctypes binding / in-tree nvcc build of lib/libb200rec.so
   ops.py           torch wrappers of the C ABI + autograd glue (SelectedRows gradients)
   nn.py            Embedding / Linear with Paddle's semantics

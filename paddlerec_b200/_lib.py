@@ -19,7 +19,7 @@ LIB_PATH = os.path.join(LIB_DIR, "libb200rec.so")
 INCLUDE_DIR = os.path.join(REPO_ROOT, "include")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC",
 ]
 
@@ -44,7 +44,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/b200rec.cu for sm_100a into paddlerec_b200/lib/libb200rec.so (in-tree)."""
+    """Compile csrc/b200rec.cu for sm_90a (H100) into paddlerec_b200/lib/libb200rec.so (in-tree)."""
     if not force and not needs_build():
         return LIB_PATH
     nvcc = os.environ.get("NVCC", "nvcc")

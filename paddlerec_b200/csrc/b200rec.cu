@@ -1,5 +1,5 @@
 // libb200rec.so — the single translation unit behind include/b200rec.h.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -shared -Xcompiler -fPIC
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared -Xcompiler -fPIC
 #include <stdarg.h>
 #include <string.h>
 
@@ -37,7 +37,7 @@ int sm_count() {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       cached = n;
     else
-      cached = 148;
+      cached = 132;
   }
   return cached;
 }
@@ -303,7 +303,7 @@ int b200rec_tower_relu_bwd_split(const float* dy, const void* act_bf16, void* dz
                                      workspace_bytes, ST(stream));
 }
 
-/* ---- tcgen05 tower GEMMs (csrc/tc_gemm.cuh) ------------------------------------------------ */
+/* ---- wgmma tower GEMMs (csrc/tc_gemm.cuh) ------------------------------------------------ */
 int b200rec_tc_split(const float* x, int64_t ldx, const float* bias, int relu, void* planes,
                      int64_t ldp, int64_t M, int K, int ones_col, void* stream) {
   if (M > 0) { NOT_NULL(x); NOT_NULL(planes); }
@@ -537,8 +537,6 @@ int b200rec_tc_debug(int key, int value) {
     case 2: tc::g_dw_debug.lbo_b = (uint32_t)value; break;
     case 3: tc::g_dw_debug.sbo = (uint32_t)value; break;
     case 4: tc::g_bk = value == 32 ? 32 : 64; break;
-    case 5: tc::g_tma_store = value != 0; break;
-    case 6: tc::g_two_cta = value != 0; break;
     default: set_error("tc_debug: unknown key %d", key); return B200REC_ERR_INVALID;
   }
   return B200REC_OK;

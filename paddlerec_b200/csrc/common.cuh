@@ -1,4 +1,4 @@
-// Shared helpers for the b200rec kernels (sm_100a only).
+// Shared helpers for the b200rec kernels (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -37,7 +37,7 @@ static inline bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// B200: 148 SMs.  Queried once; used to size persistent grids.
+// H100 SXM: 132 SMs.  Queried once; used to size persistent grids.
 int sm_count();
 
 // out-of-range id counter.  The library is ONE translation unit (b200rec.cu includes every

@@ -39,7 +39,7 @@ cross_v2_fwd_kernel(const float* __restrict__ x0, const float* __restrict__ xl,
 // Each thread owns one column chunk and walks a strided slice of rows, so the bias column-sum is
 // a register accumulation; partial sums per row-slice go to the workspace and are added in a
 // fixed order by reduce_partials_kernel (deterministic).
-constexpr int kCrossRowSlices = 148 * 2;
+constexpr int kCrossRowSlices = 132 * 2;
 
 template <int VEC>
 __global__ void __launch_bounds__(kCrossThreads)

@@ -100,7 +100,7 @@ __global__ void auc_update_kernel(const float* __restrict__ pred, const LabelT* 
   atomicAdd(reinterpret_cast<unsigned long long*>(is_pos ? pos : neg) + b, 1ull);
 }
 
-constexpr int kLossBlocks = 148;
+constexpr int kLossBlocks = 132;
 static size_t log_loss_ws_bytes() { return (size_t)kLossBlocks * sizeof(float) + 16; }
 
 }  // namespace b200rec

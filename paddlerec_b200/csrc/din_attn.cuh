@@ -8,7 +8,7 @@
 // formulation) and the t-term  tb = t (Wb-Wc) + b1  is one [B,E]x[E,80] GEMM done once per sample
 // by the caller.  FLOP-bound (2*L*(2E*80 + 80*40 + 40) flop per sample, 4.8 MFLOP at L=100) on the
 // fp32 SIMT pipe: this round's kernel is a register-tiled shared-memory GEMM, not tensor-core code
-// (the 1e-4 parity bar rules out single-pass TF32/BF16; a split-precision tcgen05 version is listed
+// (the 1e-4 parity bar rules out single-pass TF32/BF16; a split-precision wgmma version is listed
 // in DESIGN.md as next).
 //
 //   kernel A (din_scores_kernel): persistent CTAs over tiles of 64 flattened (b,l) positions;

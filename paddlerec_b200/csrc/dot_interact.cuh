@@ -121,11 +121,11 @@ dot_interact_bwd_kernel(const float* __restrict__ T, const float* __restrict__ d
 
 // ================================================================================================
 // v2 — EXPERIMENTAL, opt-in with B200REC_K6_V2=1 (d % 4 == 0).  Written after the round's GPU budget
-// was spent: it compiles for sm_100a but has NOT run on hardware yet; the default path above is the
+// was spent: it compiles for sm_90a but has NOT run on hardware yet; the default path above is the
 // validated one.  Parity test: tests/test_gpu_kernels.py::test_dot_interact_v2_matches_v1 (enabled
 // with B200REC_TEST_EXPERIMENTAL=1); timing: tools/dot_bench.py --v2.
 //
-// What the v1 measurement said (profiles/r1j_dot_interact_bench.jsonl: 0.20 of HBM peak forward):
+// What the v1 measurement said (0.20 of HBM peak forward, on the GPU the project first targeted):
 // ~530 warp instructions per sample, two scalar shared-memory loads per FMA, and no overlap between
 // a warp's global loads and its math.  v2 changes exactly those two things:
 //   * rows live at a pitch of d+4 floats, so every row is 16-byte aligned and the inner product

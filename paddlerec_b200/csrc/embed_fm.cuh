@@ -346,10 +346,10 @@ embed_fm_fwd_warp_kernel(const float* __restrict__ W, const float* __restrict__ 
 //     waits for it (wait_group.read) right before it overwrites the tile for its next iteration —
 //     the second CTA of the SM gathers meanwhile.
 // ids/dense of the next tile are prefetched with cp.async into a second small buffer.
-// STATUS (round 1): correct (same tests as the register variant) but slower — 0.141 ms vs 0.092 ms
-// at B=65536, D=16: one 32-sample tile is 80 KB, so only 2 CTAs = 8 warps fit per SM and the
-// per-field issue chain (LDS id -> compare -> address -> LDGSTS) is not hidden (ncu:
-// profiles/r1g_k1_tma_variant.txt).  Opt-in with B200REC_K1_TMA=1; the register variant is default.
+// STATUS: correct (same tests as the register variant) but it was slower where it was measured
+// (on the GPU the project first targeted; not re-measured on the H100): one 32-sample tile is
+// 80 KB, so only 2 CTAs = 8 warps fit per SM and the per-field issue chain (LDS id -> compare ->
+// address -> LDGSTS) is not hidden.  Opt-in with B200REC_K1_TMA=1; the register variant is default.
 constexpr int kTmaThreads = 128;
 
 __device__ __forceinline__ void cp_async_16_cg(void* smem, const void* gmem) {

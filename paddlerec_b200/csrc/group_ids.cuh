@@ -7,7 +7,7 @@
 //   head flags -> inclusive scan -> segment table
 //
 // The radix sort and the scan are CUB device primitives (shipped with the CUDA toolkit and
-// compiled here for sm_100a); the key building and segment-table kernels are ours.
+// compiled here for sm_90a); the key building and segment-table kernels are ours.
 #pragma once
 
 #include <cub/device/device_radix_sort.cuh>

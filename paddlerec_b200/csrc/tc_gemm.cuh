@@ -1,30 +1,31 @@
-// Hand-written tcgen05 / TMEM / TMA GEMMs for the dense tower in split precision ("bf16x3").
+// Hand-written wgmma / TMA GEMMs for the dense tower in split precision ("bf16x3").
 //
 // Reference path: DNN.forward models/rank/deepfm/net.py:169-174 (Linear -> ReLU chain), its autograd
 // (tools/trainer.py:151 loss.backward()), and the same chain in dcn_v2/net.py:178-184,
-// wide_deep/net.py:95-97, din/net.py:175-184.  An fp32 product a@w is evaluated on the 5th-gen
+// wide_deep/net.py:95-97, din/net.py:175-184.  An fp32 product a@w is evaluated on the Hopper
 // tensor cores as a_hi@w_hi + a_lo@w_hi + a_hi@w_lo (bf16 operands, exact products, fp32
-// accumulation in TMEM; ~2^-16 relative), which meets the 1e-4 logit bar that plain TF32 misses.
+// accumulation in registers; ~2^-16 relative), which meets the 1e-4 logit bar that plain TF32 misses.
 //
 // Operand format ("planes"): a matrix X[R, C] lives in HBM as bf16 [R, 2*ld] with the rounded value
 // hi(X) in columns [0, C) and the residual lo(X) = bf16(X - hi) in columns [ld, ld + C); ld is C
 // rounded up to 8 so that both planes are 16-byte aligned TMA tensors.  Same bytes as fp32.
 //
-// Two kernels, both warp-specialised (warp 0 = TMA producer, warp 1 = tcgen05.mma issuer and TMEM
-// owner, warps 2-5 = epilogue) with mbarrier pipelines smem full/empty and TMEM full/empty:
+// Two kernels, both warp-specialised over three warpgroups (warpgroup 0 = TMA producer, warpgroups
+// 1 and 2 = wgmma.mma_async consumers owning 64 output rows each, fp32 accumulators in registers)
+// with an mbarrier pipeline full/empty over the shared-memory stages:
 //
 //   tc_gemm_kmajor_kernel   D[M,N] = A[M,K] . B[N,K]^T     both operands K-major (reduction dim
 //       contiguous): forward (A = activations, B = W^T planes) and dX (A = dZ planes, B = W
-//       planes).  Persistent over 128 x BN output tiles, two TMEM accumulator stages so the
-//       epilogue of tile t overlaps the main loop of tile t+1.  Fused epilogues: +bias, ReLU,
-//       hi/lo split (emits the NEXT GEMM's operand directly), ReLU mask + bias column-sum in
-//       backward, or plain fp32.
+//       planes).  Persistent over 128 x BN output tiles; the producer streams the next tile's
+//       k-blocks while the consumers run the epilogue of the current one.  Fused epilogues, straight
+//       from the accumulator registers: +bias, ReLU, hi/lo split (emits the NEXT GEMM's operand
+//       directly), ReLU mask + bias column-sum in backward, or plain fp32.
 //   tc_gemm_dw_kernel       dW[K,N] = sum_m A[m,K] . G[m,N]   both operands MN-major (the batch dim
-//       is the reduction), split over the batch across CTAs, fp32 partial tiles + fixed-order
-//       reduce (deterministic, no atomics).
+//       is the reduction; wgmma reads both transposed), split over the batch across CTAs, fp32
+//       partial tiles + fixed-order reduce (deterministic, no atomics).
 //
-// Shared-memory tiles are 128-byte-swizzled exactly as TMA writes them (CU_TENSOR_MAP_SWIZZLE_128B)
-// and described to the tensor core by 64-bit UMMA descriptors (layout type SWIZZLE_128B, version 1).
+// Shared-memory tiles are swizzled exactly as TMA writes them (CU_TENSOR_MAP_SWIZZLE_128B, or 64B
+// for 32-wide k-blocks) and described to wgmma by 64-bit shared-memory matrix descriptors.
 #pragma once
 
 #include <cuda.h>  // CUtensorMap and enums only; cuTensorMapEncodeTiled is resolved at run time
@@ -35,17 +36,12 @@
 namespace b200rec {
 namespace tc {
 
-constexpr int kBM = 128;         // output rows per tile = UMMA M (cta_group::1)
-constexpr int kBK = 64;          // bf16 per k-block = one 128-byte swizzle row
-constexpr int kUK = 16;          // UMMA K for 16-bit operands
-constexpr int kThreads = 192;    // dW kernel: warp 0 TMA, warp 1 MMA, warps 2..5 epilogue
-constexpr int kEpiWarps = 8;     // K-major kernel: two epilogue warpgroups (alternate 32-col chunks)
-constexpr int kThreadsK = 64 + 32 * kEpiWarps;
-constexpr uint32_t kStagingPerWarp = 4096;   // one 32x32 chunk: hi + lo bf16 tiles, or one fp32 tile
-constexpr int kTmemCols = 512;   // whole TMEM of the SM (one CTA per SM by shared-memory size)
-constexpr int kAccStride = 256;  // column offset of the second accumulator stage
-constexpr int kMaxBN = 256;
-constexpr int kDwBR = 32;        // batch rows per k-block of the dW kernel
+constexpr int kBM = 128;          // output rows per tile: two consumer warpgroups x wgmma M = 64
+constexpr int kUK = 16;           // wgmma K for 16-bit operands
+constexpr int kThreads = 384;     // warpgroup 0: TMA producer; warpgroups 1, 2: wgmma + epilogue
+constexpr int kConsumerWarps = 8;
+constexpr int kMaxBN = 256;       // wgmma N limit; the accumulator is BN / 2 registers per thread
+constexpr int kDwBR = 32;         // batch rows per k-block of the dW kernel
 constexpr uint32_t kSmemBudget = 227u * 1024u - 2048u;
 
 // device-side error word: a pipeline wait that exceeds its budget records where and traps, so a
@@ -96,7 +92,7 @@ __device__ __forceinline__ void fence_barrier_init() {
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory");
 }
-// 2-D tiled TMA load: box lands in shared memory 128B-swizzled, completion on an mbarrier.
+// 2-D tiled TMA load: box lands in shared memory swizzled, completion on an mbarrier.
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, uint32_t bar,
                                             int x, int y) {
   asm volatile(
@@ -105,136 +101,179 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, 
       "l"(m), "r"(bar), "r"(x), "r"(y)
       : "memory");
 }
-
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// all tcgen05.mma issued so far by this thread -> one arrival on `bar` when they complete
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   bar)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] . B[smem desc], bf16 x bf16 -> fp32
-__device__ __forceinline__ void tc_mma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                       uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// ---- cta_group::2 (CTA pair) variants ----------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap* m, uint32_t bar,
-                                                int x, int y) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(m), "r"(bar), "r"(x), "r"(y)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma2(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrival on the barrier at the same offset in BOTH CTAs of the pair
-__device__ __forceinline__ void tc_commit2(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], %1;" ::"r"(bar),
-      "h"((uint16_t)3)
-      : "memory");
-}
-// arrive on the barrier at local offset `bar` in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(rank));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote)
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp gets row (lane base + t)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+// at most N committed wgmma groups of this warpgroup still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// the accumulator registers are written asynchronously: keep the compiler from moving their reads
+// (the epilogue) above the wgmma_wait that completes them
+template <int R>
+__device__ __forceinline__ void fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // ------------------------------------------------------------------------------------------------
 // descriptors
 // ------------------------------------------------------------------------------------------------
-// UMMA shared-memory descriptor, SWIZZLE_128B (bits: [0,14) addr>>4, [16,30) LBO>>4, [32,46)
-// SBO>>4, [46,48) version = 1 on sm_100, [61,64) layout type = 2).
-// layout: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes,
-                                              uint32_t sbo_bytes, uint32_t layout = 2u) {
+// wgmma shared-memory matrix descriptor (bits: [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4,
+// [62,64) swizzle: 1 = 128B, 2 = 64B).  K-major: SBO = stride between 8-row groups, LBO unused
+// (one swizzle row spans the whole k-block).  MN-major: LBO = stride between 64-element column
+// chunks, SBO = stride between 8-row (k) groups.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes,
+                                              uint32_t sbo_bytes, uint32_t layout) {
   return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)layout << 61);
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | ((uint64_t)layout << 62);
 }
-// instruction descriptor for kind::f16: fp32 accumulate, bf16 x bf16, M = 128, N = n
-__host__ __device__ inline uint32_t umma_idesc(int n, int a_mn_major, int b_mn_major,
-                                               int m = 128) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(a_mn_major & 1) << 15) |
-         ((uint32_t)(b_mn_major & 1) << 16) | ((uint32_t)(n >> 3) << 17) |
-         ((uint32_t)(m >> 4) << 24);
-}
+
+// wgmma.mma_async m64nNk16, bf16 x bf16 -> fp32: d (N / 2 registers per thread) += A . B with both
+// operands read from shared memory through descriptors; TA / TB = 1: the operand is stored
+// MN-major.  acc = 0 overwrites d instead of accumulating.
+template <int N, int TA, int TB>
+struct Wgmma;
+
+template <int TA, int TB>
+struct Wgmma<16, TA, TB> {
+  static __device__ __forceinline__ void mma(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7"
+        "}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7])
+        : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+  }
+};
+
+template <int TA, int TB>
+struct Wgmma<64, TA, TB> {
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
+        "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]),
+          "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]),
+          "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]),
+          "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+  }
+};
+
+template <int TA, int TB>
+struct Wgmma<128, TA, TB> {
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
+        "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, "
+        "%34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, "
+        "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]),
+          "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]),
+          "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]),
+          "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]),
+          "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]),
+          "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]),
+          "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]),
+          "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+  }
+};
+
+template <int TA, int TB>
+struct Wgmma<208, TA, TB> {
+  static __device__ __forceinline__ void mma(float (&d)[104], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %106, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n208k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
+        "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, "
+        "%34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, "
+        "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, "
+        "%66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, "
+        "%82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, "
+        "%98, %99, %100, %101, %102, %103"
+        "}, %104, %105, p, 1, 1, %107, %108;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]),
+          "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]),
+          "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]),
+          "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]),
+          "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]),
+          "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]),
+          "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]),
+          "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]),
+          "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]),
+          "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]),
+          "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]),
+          "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]),
+          "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103])
+        : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+  }
+};
+
+template <int TA, int TB>
+struct Wgmma<256, TA, TB> {
+  static __device__ __forceinline__ void mma(float (&d)[128], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
+        "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, "
+        "%34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, "
+        "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, "
+        "%66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, "
+        "%82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, "
+        "%98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, "
+        "%111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, "
+        "%124, %125, %126, %127"
+        "}, %128, %129, p, 1, 1, %131, %132;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]),
+          "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]),
+          "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]),
+          "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]),
+          "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]),
+          "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]),
+          "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]),
+          "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]),
+          "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]),
+          "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]),
+          "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]),
+          "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]),
+          "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]),
+          "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]),
+          "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]),
+          "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+  }
+};
 
 // ------------------------------------------------------------------------------------------------
 // epilogue description (plain pointers: this struct crosses into the kernel by value)
@@ -256,9 +295,6 @@ struct Epilogue {
   // also write out_planes[m, N] = 1.0 (hi) / 0 (lo): the column of ones that makes the dW GEMM of
   // the next layer produce its bias gradient as row N (needs ldp > N)
   int ones_col;
-  // outputs that leave the SM as TMA bulk stores of swizzled shared-memory tiles (host decides:
-  // needs 16-byte aligned base and pitch; at most one of the two uses the staging buffer)
-  int tma_planes, tma_f32;
   const float* addend;              // [M, ld_add] added to acc (+bias) before everything else, or null
   int64_t ld_add;
   float* aux_f32;                   // [M, ld_aux] receives acc + bias + addend, i.e. the value BEFORE
@@ -271,24 +307,6 @@ __device__ __forceinline__ void split_bf16(float x, float& hi_f, __nv_bfloat16& 
   hi_f = __bfloat162float(hi);
   lo = __float2bfloat16_rn(x - hi_f);
 }
-__device__ __forceinline__ uint32_t pack_bf16(__nv_bfloat16 a, __nv_bfloat16 b) {
-  return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
-}
-
-// sum of v[j] over the 32 lanes for every j: 31 shuffles; lane j ends with column j's total
-__device__ __forceinline__ float warp_transpose_sum(float (&v)[32], int lane) {
-#pragma unroll
-  for (int h = 16; h >= 1; h >>= 1) {
-    const bool up = (lane & h) != 0;
-#pragma unroll
-    for (int i = 0; i < h; ++i) {
-      const float send = up ? v[i] : v[i + h];
-      const float keep = up ? v[i + h] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, h);
-    }
-  }
-  return v[0];
-}
 
 // hi/lo split of two values, packed for a 32-bit store (element a at the lower address)
 __device__ __forceinline__ void split_pack2(float a, float b, uint32_t& hi, uint32_t& lo) {
@@ -299,320 +317,178 @@ __device__ __forceinline__ void split_pack2(float a, float b, uint32_t& hi, uint
   lo = *reinterpret_cast<const uint32_t*>(&l2);
 }
 
-// ---- staged outputs: the warp's 32x32 chunk is written to shared memory in the swizzled layout
-// the TMA engine expects and leaves as ONE bulk tensor store per plane (coalesced, asynchronous,
-// no L1 involvement; rows/columns outside the matrix are clipped by the tensor map).
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src, int x, int y) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(m),
-               "r"(src), "r"(x), "r"(y)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() {
-  asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-}
-__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c,
-                                             uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d)
-               : "memory");
-}
-// 32 rows x 32 bf16 (64-byte rows, SWIZZLE_64B): hi tile at sbuf, lo tile at sbuf + 2048
-__device__ __forceinline__ void stage_planes(uint32_t sbuf, int lane, const float (&v)[32]) {
-  const uint32_t rowoff = (uint32_t)lane * 64u;
-  const uint32_t sw = ((uint32_t)lane >> 1) & 3u;
-#pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    uint32_t h[4], l[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) split_pack2(v[8 * g + 2 * j], v[8 * g + 2 * j + 1], h[j], l[j]);
-    const uint32_t off = rowoff + (((uint32_t)g ^ sw) << 4);
-    st_shared_v4(sbuf + off, h[0], h[1], h[2], h[3]);
-    st_shared_v4(sbuf + 2048u + off, l[0], l[1], l[2], l[3]);
+__device__ __forceinline__ bool al8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
+__device__ __forceinline__ bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
+
+// p[0], p[1] (the second only if `two`): one 64-bit access where the address allows it
+__device__ __forceinline__ void ld_pair(const float* p, bool two, float& x, float& y) {
+  if (two && al8(p)) {
+    const float2 v = __ldg(reinterpret_cast<const float2*>(p));
+    x = v.x; y = v.y;
+  } else {
+    x = __ldg(p);
+    y = two ? __ldg(p + 1) : 0.f;
   }
 }
-// 32 rows x 32 fp32 (128-byte rows, SWIZZLE_128B) at sbuf
-__device__ __forceinline__ void stage_f32(uint32_t sbuf, int lane, const float (&v)[32]) {
-  const uint32_t rowoff = (uint32_t)lane * 128u;
-  const uint32_t sw = (uint32_t)lane & 7u;
-#pragma unroll
-  for (int g = 0; g < 8; ++g)
-    st_shared_v4(sbuf + rowoff + (((uint32_t)g ^ sw) << 4), __float_as_uint(v[4 * g]),
-                 __float_as_uint(v[4 * g + 1]), __float_as_uint(v[4 * g + 2]),
-                 __float_as_uint(v[4 * g + 3]));
+__device__ __forceinline__ void st_pair(float* p, bool two, float x, float y) {
+  if (two && al8(p)) {
+    *reinterpret_cast<float2*>(p) = make_float2(x, y);
+  } else {
+    p[0] = x;
+    if (two) p[1] = y;
+  }
+}
+__device__ __forceinline__ void st_pair_bf16(__nv_bfloat16* p, bool two, uint32_t packed) {
+  if (two && al4(p)) {
+    *reinterpret_cast<uint32_t*>(p) = packed;
+  } else {
+    p[0] = __ushort_as_bfloat16((unsigned short)(packed & 0xFFFFu));
+    if (two) p[1] = __ushort_as_bfloat16((unsigned short)(packed >> 16));
+  }
 }
 
-// Full 32-column chunk, everything 16-byte aligned: vector loads/stores only.  `mk` holds the 32
-// mask values (bf16 pairs) fetched before the TMEM wait.
-__device__ __forceinline__ void epilogue_fast(const Epilogue& ep, float (&v)[32], int64_t row,
-                                              int col0, const uint4 (&mk)[4], bool store_f32,
-                                              bool store_planes) {
+// The two horizontally adjacent accumulator values (row, col) and (row, col + 1) of one thread ->
+// outputs; returns the emitted values.  `two`: column col + 1 exists in the matrix (else b is
+// dropped and returned as 0, so that column sums stay exact).  The caller skips rows outside the
+// matrix.  Not inlined on purpose: the tile epilogue calls it BN / 4 times per thread, and inlined
+// copies of this body for a 256-wide tile outgrow the instruction cache (measured: the K-major
+// GEMM at BN = 256 ran at a fifth of the dW kernel's rate).
+__device__ __noinline__ float2 epilogue_pair(const Epilogue& ep, float a, float b, int64_t row,
+                                             int col, bool two) {
+  float x, y;
   if (ep.bias != nullptr) {
-#pragma unroll
-    for (int g = 0; g < 8; ++g) {
-      const float4 b = __ldg(reinterpret_cast<const float4*>(ep.bias + col0) + g);
-      v[4 * g] += b.x; v[4 * g + 1] += b.y; v[4 * g + 2] += b.z; v[4 * g + 3] += b.w;
-    }
+    ld_pair(ep.bias + col, two, x, y);
+    a += x; b += y;
   }
   if (ep.addend != nullptr) {
-    const float4* ad = reinterpret_cast<const float4*>(ep.addend + row * ep.ld_add + col0);
-#pragma unroll
-    for (int g = 0; g < 8; ++g) {
-      const float4 a = __ldg(ad + g);
-      v[4 * g] += a.x; v[4 * g + 1] += a.y; v[4 * g + 2] += a.z; v[4 * g + 3] += a.w;
-    }
+    ld_pair(ep.addend + row * ep.ld_add + col, two, x, y);
+    a += x; b += y;
   }
-  if (ep.aux_f32 != nullptr) {
-    float4* o = reinterpret_cast<float4*>(ep.aux_f32 + row * ep.ld_aux + col0);
-#pragma unroll
-    for (int g = 0; g < 8; ++g) o[g] = make_float4(v[4 * g], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
-  }
+  if (ep.aux_f32 != nullptr) st_pair(ep.aux_f32 + row * ep.ld_aux + col, two, a, b);
   if (ep.cross_x0 != nullptr) {
-    const float4* x0 = reinterpret_cast<const float4*>(ep.cross_x0 + row * ep.ld_cross + col0);
-    const float4* xl = reinterpret_cast<const float4*>(ep.cross_xl + row * ep.ld_cross + col0);
-#pragma unroll
-    for (int g = 0; g < 8; ++g) {
-      const float4 a = __ldg(x0 + g), b = __ldg(xl + g);
-      v[4 * g] = fmaf(a.x, v[4 * g], b.x);
-      v[4 * g + 1] = fmaf(a.y, v[4 * g + 1], b.y);
-      v[4 * g + 2] = fmaf(a.z, v[4 * g + 2], b.z);
-      v[4 * g + 3] = fmaf(a.w, v[4 * g + 3], b.w);
-    }
+    float z, w;
+    ld_pair(ep.cross_x0 + row * ep.ld_cross + col, two, x, y);
+    ld_pair(ep.cross_xl + row * ep.ld_cross + col, two, z, w);
+    a = fmaf(x, a, z);
+    b = fmaf(y, b, w);
   }
   if (ep.relu) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+    a = fmaxf(a, 0.f);
+    b = fmaxf(b, 0.f);
   }
   if (ep.mask_src != nullptr) {
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const uint32_t w[4] = {mk[g].x, mk[g].y, mk[g].z, mk[g].w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        // bf16 > 0  <=>  its bit pattern, as a signed integer in the high half, is > 0
-        if (!((int)(w[j] << 16) > 0)) v[8 * g + 2 * j] = 0.f;
-        if (!((int)(w[j] & 0xFFFF0000u) > 0)) v[8 * g + 2 * j + 1] = 0.f;
-      }
-    }
+    const __nv_bfloat16* m = ep.mask_src + row * ep.ld_mask + col;
+    // bf16 > 0  <=>  its bit pattern, as a signed integer in the high half, is > 0
+    uint32_t w;
+    if (two && al4(m))
+      w = __ldg(reinterpret_cast<const unsigned int*>(m));
+    else
+      w = (uint32_t)__bfloat16_as_ushort(m[0]) |
+          (two ? (uint32_t)__bfloat16_as_ushort(m[1]) << 16 : 0u);
+    if (!((int)(w << 16) > 0)) a = 0.f;
+    if (!((int)(w & 0xFFFF0000u) > 0)) b = 0.f;
   }
-  if (ep.out_f32 != nullptr && store_f32) {
-    float4* o = reinterpret_cast<float4*>(ep.out_f32 + row * ep.ld_f32 + col0);
-#pragma unroll
-    for (int g = 0; g < 8; ++g) o[g] = make_float4(v[4 * g], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
+  if (!two) b = 0.f;
+  if (ep.out_f32 != nullptr) st_pair(ep.out_f32 + row * ep.ld_f32 + col, two, a, b);
+  if (ep.out_planes != nullptr) {
+    __nv_bfloat16* oh = ep.out_planes + row * 2 * ep.ldp + col;
+    uint32_t h, l;
+    split_pack2(a, b, h, l);
+    st_pair_bf16(oh, two, h);
+    st_pair_bf16(oh + ep.ldp, two, l);
   }
-  if (ep.out_planes != nullptr && store_planes) {
-    uint4* oh = reinterpret_cast<uint4*>(ep.out_planes + row * 2 * ep.ldp + col0);
-    uint4* ol = reinterpret_cast<uint4*>(ep.out_planes + row * 2 * ep.ldp + ep.ldp + col0);
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      uint32_t h[4], l[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) split_pack2(v[8 * g + 2 * j], v[8 * g + 2 * j + 1], h[j], l[j]);
-      oh[g] = make_uint4(h[0], h[1], h[2], h[3]);
-      ol[g] = make_uint4(l[0], l[1], l[2], l[3]);
-    }
-  }
+  return make_float2(a, b);
 }
 
-// One row (this thread) x 32 columns of the accumulator -> outputs.  n_valid = columns of this chunk
-// that exist in the matrix; row_ok = the row exists.
-__device__ __forceinline__ void epilogue_chunk(const Epilogue& ep, float (&v)[32], int64_t row,
-                                               bool row_ok, int col0, int n_valid, int lane,
-                                               float* s_colsum /* [32] for this warp or null */,
-                                               bool store_f32 = true, bool store_planes = true) {
-  if (ep.bias != nullptr || ep.cross_x0 != nullptr || ep.relu || ep.mask_src != nullptr ||
-      ep.addend != nullptr || ep.aux_f32 != nullptr) {
+// One consumer thread's share of a 128 x BN accumulator tile -> outputs.  wgmma m64nN layout: the
+// thread holds rows r0 = 16 * (warp in warpgroup) + lane / 4 and r0 + 8 of its warpgroup's 64 rows,
+// columns 8 j + 2 (lane % 4) + {0, 1}: acc[4j], acc[4j + 1] on row r0, acc[4j + 2], acc[4j + 3] on
+// row r0 + 8.  With s_colsum ([8 consumer warps][kMaxBN]) the warp's column sums of the emitted
+// values land there (fixed-order shuffle tree: deterministic).
+template <int BN>
+__device__ __forceinline__ void epilogue_tile(const Epilogue& ep, float (&acc)[BN / 2], int M,
+                                              int N, int m0, int n0, int cw, int lane,
+                                              float* s_colsum) {
+  const int64_t r0 = (int64_t)m0 + 16 * cw + (lane >> 2);
+  const bool ok0 = r0 < M, ok1 = r0 + 8 < M;
 #pragma unroll
-    for (int g = 0; g < 8; ++g) {   // groups of 4 columns
-      const int c = g * 4;
-      if (c < n_valid) {
-        if (ep.bias != nullptr) {
-          if (c + 4 <= n_valid && (reinterpret_cast<uintptr_t>(ep.bias + col0 + c) & 15u) == 0) {
-            const float4 b = __ldg(reinterpret_cast<const float4*>(ep.bias + col0 + c));
-            v[c] += b.x; v[c + 1] += b.y; v[c + 2] += b.z; v[c + 3] += b.w;
-          } else {
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = n0 + 8 * j + 2 * (lane & 3);
+    const bool in = col < N, two = col + 1 < N;
+    float2 v0 = make_float2(0.f, 0.f), v1 = make_float2(0.f, 0.f);
+    if (in && ok0) v0 = epilogue_pair(ep, acc[4 * j], acc[4 * j + 1], r0, col, two);
+    if (in && ok1) v1 = epilogue_pair(ep, acc[4 * j + 2], acc[4 * j + 3], r0 + 8, col, two);
+    acc[4 * j] = v0.x; acc[4 * j + 1] = v0.y; acc[4 * j + 2] = v1.x; acc[4 * j + 3] = v1.y;
+    if (s_colsum != nullptr) {
+      float s0 = acc[4 * j] + acc[4 * j + 2], s1 = acc[4 * j + 1] + acc[4 * j + 3];
 #pragma unroll
-            for (int j = 0; j < 4; ++j)
-              if (c + j < n_valid) v[c + j] += __ldg(ep.bias + col0 + c + j);
-          }
-        }
-        if (ep.addend != nullptr && row_ok) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (c + j < n_valid) v[c + j] += __ldg(ep.addend + row * ep.ld_add + col0 + c + j);
-        }
-        if (ep.aux_f32 != nullptr && row_ok) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (c + j < n_valid) ep.aux_f32[row * ep.ld_aux + col0 + c + j] = v[c + j];
-        }
-        if (ep.cross_x0 != nullptr && row_ok) {
-          const float* x0 = ep.cross_x0 + row * ep.ld_cross + col0 + c;
-          const float* xl = ep.cross_xl + row * ep.ld_cross + col0 + c;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (c + j < n_valid) v[c + j] = fmaf(__ldg(x0 + j), v[c + j], __ldg(xl + j));
-        }
-        if (ep.relu) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) v[c + j] = fmaxf(v[c + j], 0.f);
-        }
+      for (int h = 4; h <= 16; h <<= 1) {
+        s0 += __shfl_xor_sync(0xffffffffu, s0, h);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, h);
       }
-    }
-    if (ep.mask_src != nullptr) {
-      const __nv_bfloat16* mrow = ep.mask_src + row * ep.ld_mask + col0;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {   // groups of 8 columns = 16 bytes of bf16
-        const int c = g * 8;
-        if (c + 8 <= n_valid && row_ok && (reinterpret_cast<uintptr_t>(mrow + c) & 15u) == 0) {
-          const uint4 q = __ldg(reinterpret_cast<const uint4*>(mrow + c));
-          const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float a0 = __uint_as_float(w[j] << 16);
-            const float a1 = __uint_as_float(w[j] & 0xFFFF0000u);
-            if (!(a0 > 0.f)) v[c + 2 * j] = 0.f;
-            if (!(a1 > 0.f)) v[c + 2 * j + 1] = 0.f;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            if (c + j < n_valid && row_ok) {
-              if (!(__bfloat162float(mrow[c + j]) > 0.f)) v[c + j] = 0.f;
-            }
-        }
+      if (lane < 4) {
+        s_colsum[8 * j + 2 * lane] = s0;
+        s_colsum[8 * j + 2 * lane + 1] = s1;
       }
     }
   }
-  if (!row_ok) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = 0.f;
-  }
-  if (row_ok) {
-    if (ep.out_f32 != nullptr && store_f32) {
-      float* o = ep.out_f32 + row * ep.ld_f32 + col0;
-      const bool vec_ok = (reinterpret_cast<uintptr_t>(o) & 15u) == 0;
-#pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        const int c = g * 4;
-        if (c + 4 <= n_valid && vec_ok) {
-          *reinterpret_cast<float4*>(o + c) = make_float4(v[c], v[c + 1], v[c + 2], v[c + 3]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (c + j < n_valid) o[c + j] = v[c + j];
-        }
+  if (ep.ones_col && ep.out_planes != nullptr && (lane & 3) == 0 && n0 + BN >= N) {
+    for (int h = 0; h < 2; ++h) {
+      const int64_t row = r0 + 8 * h;
+      if (row < M) {
+        __nv_bfloat16* oh = ep.out_planes + row * 2 * ep.ldp + N;
+        oh[0] = __float2bfloat16_rn(1.f);
+        oh[ep.ldp] = __float2bfloat16_rn(0.f);
       }
     }
-    if (ep.out_planes != nullptr && store_planes) {
-      __nv_bfloat16* oh = ep.out_planes + row * 2 * ep.ldp + col0;
-      __nv_bfloat16* ol = oh + ep.ldp;
-      const bool vec_ok = ((reinterpret_cast<uintptr_t>(oh) | reinterpret_cast<uintptr_t>(ol)) & 15u) == 0;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const int c = g * 8;
-        if (c >= n_valid) break;
-        __nv_bfloat16 h[8], l[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float hf;
-          split_bf16(v[c + j], hf, h[j], l[j]);
-        }
-        if (c + 8 <= n_valid && vec_ok) {
-          *reinterpret_cast<uint4*>(oh + c) = make_uint4(pack_bf16(h[0], h[1]), pack_bf16(h[2], h[3]),
-                                                         pack_bf16(h[4], h[5]), pack_bf16(h[6], h[7]));
-          *reinterpret_cast<uint4*>(ol + c) = make_uint4(pack_bf16(l[0], l[1]), pack_bf16(l[2], l[3]),
-                                                         pack_bf16(l[4], l[5]), pack_bf16(l[6], l[7]));
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            if (c + j < n_valid) {
-              oh[c + j] = h[j];
-              ol[c + j] = l[j];
-            }
-        }
-      }
-    }
-  }
-  if (s_colsum != nullptr) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (j >= n_valid) v[j] = 0.f;
-    const float t = warp_transpose_sum(v, lane);
-    s_colsum[lane] = t;
   }
 }
 
 // ------------------------------------------------------------------------------------------------
-// K-major GEMM: D[M,N] = A[M,K] . B[N,K]^T  (three tcgen05.mma per 16-wide k step)
+// K-major GEMM: D[M,N] = A[M,K] . B[N,K]^T  (three wgmma per 16-wide k step)
 //   BK = 64: 128-byte swizzle rows (2 pipeline stages at BN = 208)
 //   BK = 32: 64-byte swizzle rows, half-size stages -> 5 stages at BN = 208: same bytes in shared
 //            memory, but a freed slot is refilled twice as early, which hides the TMA latency
 // ------------------------------------------------------------------------------------------------
-template <int BK>
-__global__ void __launch_bounds__(kThreadsK, 1)
+template <int BN, int BK>
+__global__ void __launch_bounds__(kThreads, 1)
 tc_gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA_hi,
                       const __grid_constant__ CUtensorMap tmA_lo,
                       const __grid_constant__ CUtensorMap tmB_hi,
-                      const __grid_constant__ CUtensorMap tmB_lo,
-                      const __grid_constant__ CUtensorMap tmO_hi,
-                      const __grid_constant__ CUtensorMap tmO_lo,
-                      const __grid_constant__ CUtensorMap tmO_f32, int M, int N, int K, int BN,
-                      int stages, Epilogue ep) {
+                      const __grid_constant__ CUtensorMap tmB_lo, int M, int N, int K, int stages,
+                      const __grid_constant__ Epilogue ep) {
   constexpr uint32_t kRow = BK * 2;                       // bytes per operand row in a stage
-  constexpr uint32_t kLayout = BK == 64 ? 2u : 4u;        // SWIZZLE_128B / SWIZZLE_64B
+  constexpr uint32_t kLayout = BK == 64 ? 1u : 2u;        // SWIZZLE_128B / SWIZZLE_64B
   constexpr uint32_t kSbo = 8u * kRow;                    // 8-row swizzle atom
+  constexpr uint32_t a_bytes = kBM * kRow;
+  constexpr uint32_t b_bytes = BN * kRow;
+  constexpr uint32_t stage_bytes = 2u * a_bytes + 2u * b_bytes;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;          // swizzled tiles: atom-aligned
   uint8_t* sm = smem_raw + (base - raw);
-  const uint32_t a_bytes = kBM * kRow;
-  const uint32_t b_bytes = (uint32_t)BN * kRow;
-  const uint32_t stage_bytes = 2u * a_bytes + 2u * b_bytes;
-  // [stages][output staging: 4 KB per epilogue warp][barriers][tmem ptr][colsum scratch]
-  const uint32_t stage_end = (uint32_t)stages * stage_bytes;
-  const uint32_t staging = base + stage_end;
-  const uint32_t bar_off = stage_end + kEpiWarps * kStagingPerWarp;
-  const uint32_t bar0 = base + bar_off;
-  const uint32_t bar_full = bar0, bar_empty = bar0 + 8u * stages;
-  const uint32_t bar_tfull = bar0 + 16u * stages, bar_tempty = bar_tfull + 16u;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + (size_t)bar_off + 16 * stages + 32);
-  float* s_colsum = reinterpret_cast<float*>(sm + (size_t)bar_off + 16 * stages + 64);
-  // s_colsum: [4 lane quarters][kMaxBN], only with ep.colsum
+  // [stages][full barriers][empty barriers][colsum scratch: 8 warps x kMaxBN]
+  const uint32_t bar_full = base + (uint32_t)stages * stage_bytes;
+  const uint32_t bar_empty = bar_full + 8u * stages;
+  float* s_colsum = reinterpret_cast<float*>(sm + (size_t)stages * stage_bytes + 16 * stages);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_m = (M + kBM - 1) / kBM, tiles_n = (N + BN - 1) / BN;
   const int n_tiles = tiles_m * tiles_n;
   const int nkb = (K + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmB_hi); prefetch_tmap(&tmB_lo);
-    if (ep.tma_planes) { prefetch_tmap(&tmO_hi); prefetch_tmap(&tmO_lo); }
-    if (ep.tma_f32) prefetch_tmap(&tmO_f32);
     for (int s = 0; s < stages; ++s) {
       mbar_init(bar_full + 8u * s, 1);
-      mbar_init(bar_empty + 8u * s, 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(bar_tfull + 8u * s, 1);
-      mbar_init(bar_tempty + 8u * s, kEpiWarps);   // one arrival per epilogue warp
+      mbar_init(bar_empty + 8u * s, kConsumerWarps);   // one arrival per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(smem_u32(tmem_slot), kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -630,393 +506,58 @@ tc_gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA_hi,
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int n0 = (tile % tiles_n) * BN;
-        int n_cur = N - n0;
-        n_cur = n_cur >= BN ? BN : ((n_cur + 15) & ~15);
-        const uint32_t idesc = umma_idesc(n_cur, 0, 0);
-        mbar_wait(bar_tempty + 8u * acc, acc_phase ^ 1u, 0x200u + acc);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * kAccStride;
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(bar_full + 8u * stage, phase, 0x300u + stage);
-          tc_fence_after();
-          const uint32_t sA = base + (uint32_t)stage * stage_bytes;
-          const uint32_t sB = sA + 2u * a_bytes;
-          int ksteps = (K - kb * BK + kUK - 1) / kUK;
-          ksteps = ksteps > BK / kUK ? BK / kUK : ksteps;
-          for (int j = 0; j < ksteps; ++j) {
-            const uint32_t ko = (uint32_t)j * (kUK * 2);   // 32 bytes further inside the swizzle row
-            const uint64_t a_hi = umma_desc(sA + ko, 16, kSbo, kLayout);
-            const uint64_t a_lo = umma_desc(sA + a_bytes + ko, 16, kSbo, kLayout);
-            const uint64_t b_hi = umma_desc(sB + ko, 16, kSbo, kLayout);
-            const uint64_t b_lo = umma_desc(sB + b_bytes + ko, 16, kSbo, kLayout);
-            tc_mma(d_tmem, a_hi, b_hi, idesc, (kb | j) != 0 ? 1u : 0u);
-            tc_mma(d_tmem, a_lo, b_hi, idesc, 1u);
-            tc_mma(d_tmem, a_hi, b_lo, idesc, 1u);
-          }
-          tc_commit(bar_empty + 8u * stage);                 // smem slot free when these complete
-          if (kb == nkb - 1) tc_commit(bar_tfull + 8u * acc);  // accumulator ready
-          if (++stage == stages) { stage = 0; phase ^= 1u; }
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
   } else {
-    // epilogue: a warp may touch TMEM lanes 32*(warp%4) .. +31 only; the two warps that share a
-    // lane quarter take alternate 32-column chunks
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    const int cw = warp - 4;          // consumer warp 0..7; warpgroup = cw / 4 owns rows 64 (cw / 4)..
+    const int wg = cw >> 2;
     const bool want_colsum = ep.colsum != nullptr;
-    const bool tma_p = ep.tma_planes != 0 && !want_colsum, tma_f = ep.tma_f32 != 0 && !want_colsum;
-    const uint32_t sbuf = staging + (uint32_t)(warp - 2) * kStagingPerWarp;
-    const bool base_aligned =
-        (ep.out_f32 == nullptr || ((reinterpret_cast<uintptr_t>(ep.out_f32) | (ep.ld_f32 * 4)) & 15u) == 0) &&
-        (ep.out_planes == nullptr || ((reinterpret_cast<uintptr_t>(ep.out_planes) | (ep.ldp * 2)) & 15u) == 0) &&
-        (ep.mask_src == nullptr || ((reinterpret_cast<uintptr_t>(ep.mask_src) | (ep.ld_mask * 2)) & 15u) == 0) &&
-        (ep.bias == nullptr || (reinterpret_cast<uintptr_t>(ep.bias) & 15u) == 0) &&
-        (ep.addend == nullptr || ((reinterpret_cast<uintptr_t>(ep.addend) | (ep.ld_add * 4)) & 15u) == 0) &&
-        (ep.aux_f32 == nullptr || ((reinterpret_cast<uintptr_t>(ep.aux_f32) | (ep.ld_aux * 4)) & 15u) == 0) &&
-        (ep.cross_x0 == nullptr ||
-         ((reinterpret_cast<uintptr_t>(ep.cross_x0) | reinterpret_cast<uintptr_t>(ep.cross_xl) |
-           (ep.ld_cross * 4)) & 15u) == 0);
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       const int m_blk = tile / tiles_n;
       const int m0 = m_blk * kBM, n0 = (tile % tiles_n) * BN;
-      const int n_tile = (N - n0) < BN ? (N - n0) : BN;
-      const int64_t row = (int64_t)m0 + q * 32 + lane;
-      const bool row_ok = row < M;
-      // warp-uniform on purpose: tcgen05.ld is .sync.aligned, so the 32 lanes must not split into a
-      // fast and a slow path inside the chunk loop (a partially valid last row block goes slow)
-      const bool fast_ok =
-          base_aligned && ((int64_t)m0 + q * 32 + 31 < M) && (n0 & 7) == 0 && !want_colsum;
-      mbar_wait(bar_tfull + 8u * acc, acc_phase, 0x400u + acc);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * kAccStride;
-      for (int c0 = half * 32; c0 < n_tile; c0 += 64) {
-        uint32_t r[32];
-        __syncwarp();
-        tmem_ld32(t_row + (uint32_t)c0, r);
-        const int nv = (n_tile - c0) < 32 ? (n_tile - c0) : 32;
-        const bool fast = fast_ok && nv == 32;
-        uint4 mk[4];
-        if (fast && ep.mask_src != nullptr) {    // in flight while the TMEM load completes
-          const uint4* mp = reinterpret_cast<const uint4*>(ep.mask_src + row * ep.ld_mask + n0 + c0);
+      int prev = 0;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(bar_full + 8u * stage, phase, 0x300u + stage);
+        const uint32_t sA = base + (uint32_t)stage * stage_bytes + (uint32_t)wg * (64u * kRow);
+        const uint32_t sB = base + (uint32_t)stage * stage_bytes + 2u * a_bytes;
+        wgmma_fence();
 #pragma unroll
-          for (int g = 0; g < 4; ++g) mk[g] = __ldg(mp + g);
+        for (int j = 0; j < BK / kUK; ++j) {
+          const uint32_t ko = (uint32_t)j * (kUK * 2);   // 32 bytes further inside the swizzle row
+          const uint64_t a_hi = gmma_desc(sA + ko, 16, kSbo, kLayout);
+          const uint64_t a_lo = gmma_desc(sA + a_bytes + ko, 16, kSbo, kLayout);
+          const uint64_t b_hi = gmma_desc(sB + ko, 16, kSbo, kLayout);
+          const uint64_t b_lo = gmma_desc(sB + b_bytes + ko, 16, kSbo, kLayout);
+          Wgmma<BN, 0, 0>::mma(acc, a_hi, b_hi, (kb | j) != 0 ? 1u : 0u);
+          Wgmma<BN, 0, 0>::mma(acc, a_lo, b_hi, 1u);
+          Wgmma<BN, 0, 0>::mma(acc, a_hi, b_lo, 1u);
         }
-        tmem_ld_wait();
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        // Full 32-column chunks leave through the TMA staging buffer; a partial chunk (tile width
-        // not a multiple of 32) is stored directly: its 32-wide box would spill into the
-        // neighbouring tile's columns (the tensor map clips only at the matrix edge).
-        const bool via_tma = (tma_p || tma_f) && nv == 32;
-        const bool st_f = !(tma_f && via_tma), st_p = !(tma_p && via_tma);
-        if (fast)
-          epilogue_fast(ep, v, row, n0 + c0, mk, st_f, st_p);
-        else
-          epilogue_chunk(ep, v, row, row_ok, n0 + c0, nv, lane,
-                         want_colsum ? s_colsum + q * kMaxBN + c0 : nullptr, st_f, st_p);
-        if (via_tma) {
-          if (lane == 0) bulk_wait_read0();      // the previous store has finished reading sbuf
-          __syncwarp();
-          if (tma_p)
-            stage_planes(sbuf, lane, v);
-          else
-            stage_f32(sbuf, lane, v);
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            if (tma_p) {
-              tma_store_2d(&tmO_hi, sbuf, n0 + c0, m0 + q * 32);
-              tma_store_2d(&tmO_lo, sbuf + 2048u, n0 + c0, m0 + q * 32);
-            } else {
-              tma_store_2d(&tmO_f32, sbuf, n0 + c0, m0 + q * 32);
-            }
-            bulk_commit();
-          }
+        wgmma_commit();
+        if (kb > 0) {           // the previous k-block's products are done: its slot is free
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(bar_empty + 8u * prev);
         }
+        prev = stage;
+        if (++stage == stages) { stage = 0; phase ^= 1u; }
       }
-      if (ep.ones_col && ep.out_planes != nullptr && row_ok && half == 0 && n0 + n_tile == N) {
-        __nv_bfloat16* oh = ep.out_planes + row * 2 * ep.ldp + N;
-        oh[0] = __float2bfloat16_rn(1.f);
-        oh[ep.ldp] = __float2bfloat16_rn(0.f);
-      }
-      // accumulator drained -> the MMA warp may overwrite this stage
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + 8u * acc);
+      wgmma_wait<0>();
+      fence_acc(acc);
+      if (lane == 0) mbar_arrive(bar_empty + 8u * prev);
+      epilogue_tile<BN>(ep, acc, M, N, m0 + 64 * wg, n0, cw & 3, lane,
+                        want_colsum ? s_colsum + cw * kMaxBN : nullptr);
       if (want_colsum) {
-        named_bar_sync(1, 32 * kEpiWarps);
-        const int t = threadIdx.x - 64;
-        for (int c = t; c < n_tile; c += 32 * kEpiWarps) {
-          const float s = ((s_colsum[c] + s_colsum[kMaxBN + c]) + s_colsum[2 * kMaxBN + c]) +
-                          s_colsum[3 * kMaxBN + c];
+        named_bar_sync(1, 32 * kConsumerWarps);
+        const int n_tile = (N - n0) < BN ? (N - n0) : BN;
+        for (int c = threadIdx.x - 128; c < n_tile; c += 32 * kConsumerWarps) {
+          float s = 0.f;
+#pragma unroll
+          for (int w = 0; w < kConsumerWarps; ++w) s += s_colsum[w * kMaxBN + c];
           ep.colsum[(int64_t)m_blk * N + n0 + c] = s;
         }
-        named_bar_sync(1, 32 * kEpiWarps);
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-    }
-    if ((tma_p || tma_f) && lane == 0) bulk_wait0();   // shared memory must outlive the stores
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// K-major GEMM on CTA PAIRS (cta_group::2): the two SMs of a cluster compute one 256 x BN tile.
-// Each CTA loads its own 128 rows of A but only HALF of the B tile; tcgen05.mma.cta_group::2 (issued
-// by the leader CTA alone) reads B from both shared memories, so the L2 -> SM operand traffic per
-// flop drops by ~30 % (A 32 KB + B 26 KB per k-block per SM instead of 32 + 52 at BN = 208) — the
-// 1-CTA kernel above is bound by exactly that traffic — and the freed shared memory holds a third
-// pipeline stage.  Protocol (as CUTLASS's 2-SM pipelines): both producers signal the LEADER's full
-// barrier (peer bit of the barrier address cleared), the leader arms it with the bytes of both;
-// tcgen05.commit multicasts the slot release and the accumulator-ready signal to both CTAs; the
-// peer's epilogue warps arrive remotely on the leader's TMEM-empty barrier.
-// ------------------------------------------------------------------------------------------------
-template <int BK>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreadsK, 1)
-tc_gemm_kmajor2_kernel(const __grid_constant__ CUtensorMap tmA_hi,
-                      const __grid_constant__ CUtensorMap tmA_lo,
-                      const __grid_constant__ CUtensorMap tmB_hi,
-                      const __grid_constant__ CUtensorMap tmB_lo,
-                      const __grid_constant__ CUtensorMap tmO_hi,
-                      const __grid_constant__ CUtensorMap tmO_lo,
-                      const __grid_constant__ CUtensorMap tmO_f32, int M, int N, int K, int BN,
-                      int stages, Epilogue ep) {
-  constexpr uint32_t kRow = BK * 2;                       // bytes per operand row in a stage
-  constexpr uint32_t kLayout = BK == 64 ? 2u : 4u;        // SWIZZLE_128B / SWIZZLE_64B
-  constexpr uint32_t kSbo = 8u * kRow;                    // 8-row swizzle atom
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;          // swizzled tiles: atom-aligned
-  uint8_t* sm = smem_raw + (base - raw);
-  const uint32_t cta_rank = cluster_ctarank();          // 0 = leader: issues every tcgen05.mma
-  const bool leader = cta_rank == 0;
-  const int half_bn = BN / 2;                            // B rows held by EACH CTA of the pair
-  const uint32_t a_bytes = kBM * kRow;
-  const uint32_t b_bytes = (uint32_t)half_bn * kRow;
-  const uint32_t stage_bytes = 2u * a_bytes + 2u * b_bytes;
-  // [stages][output staging: 4 KB per epilogue warp][barriers][tmem ptr][colsum scratch]
-  const uint32_t stage_end = (uint32_t)stages * stage_bytes;
-  const uint32_t staging = base + stage_end;
-  const uint32_t bar_off = stage_end + kEpiWarps * kStagingPerWarp;
-  const uint32_t bar0 = base + bar_off;
-  const uint32_t bar_full = bar0, bar_empty = bar0 + 8u * stages;
-  const uint32_t bar_tfull = bar0 + 16u * stages, bar_tempty = bar_tfull + 16u;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + (size_t)bar_off + 16 * stages + 32);
-  float* s_colsum = reinterpret_cast<float*>(sm + (size_t)bar_off + 16 * stages + 64);
-  // s_colsum: [4 lane quarters][kMaxBN], only with ep.colsum
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles_m = (M + 2 * kBM - 1) / (2 * kBM), tiles_n = (N + BN - 1) / BN;   // 256-row pairs
-  const int n_tiles = tiles_m * tiles_n;
-  const int nkb = (K + BK - 1) / BK;
-  const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmB_hi); prefetch_tmap(&tmB_lo);
-    if (ep.tma_planes) { prefetch_tmap(&tmO_hi); prefetch_tmap(&tmO_lo); }
-    if (ep.tma_f32) prefetch_tmap(&tmO_f32);
-    for (int s = 0; s < stages; ++s) {
-      mbar_init(bar_full + 8u * s, 1);
-      mbar_init(bar_empty + 8u * s, 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(bar_tfull + 8u * s, 1);
-      mbar_init(bar_tempty + 8u * s, 2 * kEpiWarps);   // the epilogue warps of BOTH CTAs (leader's copy is used)
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc2(smem_u32(tmem_slot), kTmemCols);   // collective over the CTA pair (same warp id in both)
-    tmem_relinquish2();
-  }
-  tc_fence_before();
-  cluster_sync();      // barriers of both CTAs are initialised before any remote arrive / TMA signal
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = cluster_id; tile < n_tiles; tile += n_clusters) {
-        const int m0 = (tile / tiles_n) * 2 * kBM + (int)cta_rank * kBM;
-        const int n0 = (tile % tiles_n) * BN;
-        int n_cur = N - n0;
-        n_cur = n_cur >= BN ? BN : ((n_cur + 15) & ~15);
-        const int nb0 = n0 + (int)cta_rank * (n_cur / 2);     // this CTA's half of the B rows
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(bar_empty + 8u * stage, phase ^ 1u, 0x100u + stage);
-          // transaction bytes of BOTH CTAs land on the leader's barrier (peer bit cleared)
-          const uint32_t full = (bar_full + 8u * stage) & 0xFEFFFFFFu;
-          const uint32_t sA = base + (uint32_t)stage * stage_bytes;
-          if (leader) mbar_expect_tx(bar_full + 8u * stage, 2u * stage_bytes);
-          tma_load_2d_2sm(sA, &tmA_hi, full, kb * BK, m0);
-          tma_load_2d_2sm(sA + a_bytes, &tmA_lo, full, kb * BK, m0);
-          tma_load_2d_2sm(sA + 2u * a_bytes, &tmB_hi, full, kb * BK, nb0);
-          tma_load_2d_2sm(sA + 2u * a_bytes + b_bytes, &tmB_lo, full, kb * BK, nb0);
-          if (++stage == stages) { stage = 0; phase ^= 1u; }
-        }
+        named_bar_sync(1, 32 * kConsumerWarps);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int tile = cluster_id; tile < n_tiles; tile += n_clusters) {
-        const int n0 = (tile % tiles_n) * BN;
-        int n_cur = N - n0;
-        n_cur = n_cur >= BN ? BN : ((n_cur + 15) & ~15);
-        const uint32_t idesc = umma_idesc(n_cur, 0, 0, 2 * kBM);   // M = 256 over the two SMs
-        mbar_wait(bar_tempty + 8u * acc, acc_phase ^ 1u, 0x200u + acc);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * kAccStride;
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(bar_full + 8u * stage, phase, 0x300u + stage);
-          tc_fence_after();
-          const uint32_t sA = base + (uint32_t)stage * stage_bytes;
-          const uint32_t sB = sA + 2u * a_bytes;
-          int ksteps = (K - kb * BK + kUK - 1) / kUK;
-          ksteps = ksteps > BK / kUK ? BK / kUK : ksteps;
-          for (int j = 0; j < ksteps; ++j) {
-            const uint32_t ko = (uint32_t)j * (kUK * 2);   // 32 bytes further inside the swizzle row
-            const uint64_t a_hi = umma_desc(sA + ko, 16, kSbo, kLayout);
-            const uint64_t a_lo = umma_desc(sA + a_bytes + ko, 16, kSbo, kLayout);
-            const uint64_t b_hi = umma_desc(sB + ko, 16, kSbo, kLayout);
-            const uint64_t b_lo = umma_desc(sB + b_bytes + ko, 16, kSbo, kLayout);
-            tc_mma2(d_tmem, a_hi, b_hi, idesc, (kb | j) != 0 ? 1u : 0u);
-            tc_mma2(d_tmem, a_lo, b_hi, idesc, 1u);
-            tc_mma2(d_tmem, a_hi, b_lo, idesc, 1u);
-          }
-          tc_commit2(bar_empty + 8u * stage);                 // frees the slot in BOTH CTAs
-          if (kb == nkb - 1) tc_commit2(bar_tfull + 8u * acc);  // both epilogues may start
-          if (++stage == stages) { stage = 0; phase ^= 1u; }
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-  } else {
-    // epilogue: a warp may touch TMEM lanes 32*(warp%4) .. +31 only; the two warps that share a
-    // lane quarter take alternate 32-column chunks
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const bool want_colsum = ep.colsum != nullptr;
-    const bool tma_p = ep.tma_planes != 0 && !want_colsum, tma_f = ep.tma_f32 != 0 && !want_colsum;
-    const uint32_t sbuf = staging + (uint32_t)(warp - 2) * kStagingPerWarp;
-    const bool base_aligned =
-        (ep.out_f32 == nullptr || ((reinterpret_cast<uintptr_t>(ep.out_f32) | (ep.ld_f32 * 4)) & 15u) == 0) &&
-        (ep.out_planes == nullptr || ((reinterpret_cast<uintptr_t>(ep.out_planes) | (ep.ldp * 2)) & 15u) == 0) &&
-        (ep.mask_src == nullptr || ((reinterpret_cast<uintptr_t>(ep.mask_src) | (ep.ld_mask * 2)) & 15u) == 0) &&
-        (ep.bias == nullptr || (reinterpret_cast<uintptr_t>(ep.bias) & 15u) == 0) &&
-        (ep.addend == nullptr || ((reinterpret_cast<uintptr_t>(ep.addend) | (ep.ld_add * 4)) & 15u) == 0) &&
-        (ep.aux_f32 == nullptr || ((reinterpret_cast<uintptr_t>(ep.aux_f32) | (ep.ld_aux * 4)) & 15u) == 0) &&
-        (ep.cross_x0 == nullptr ||
-         ((reinterpret_cast<uintptr_t>(ep.cross_x0) | reinterpret_cast<uintptr_t>(ep.cross_xl) |
-           (ep.ld_cross * 4)) & 15u) == 0);
-    for (int tile = cluster_id; tile < n_tiles; tile += n_clusters) {
-      const int m_blk = (tile / tiles_n) * 2 + (int)cta_rank;
-      const int m0 = m_blk * kBM, n0 = (tile % tiles_n) * BN;
-      const int n_tile = (N - n0) < BN ? (N - n0) : BN;
-      const int64_t row = (int64_t)m0 + q * 32 + lane;
-      const bool row_ok = row < M;
-      // warp-uniform on purpose: tcgen05.ld is .sync.aligned, so the 32 lanes must not split into a
-      // fast and a slow path inside the chunk loop (a partially valid last row block goes slow)
-      const bool fast_ok =
-          base_aligned && ((int64_t)m0 + q * 32 + 31 < M) && (n0 & 7) == 0 && !want_colsum;
-      mbar_wait(bar_tfull + 8u * acc, acc_phase, 0x400u + acc);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * kAccStride;
-      for (int c0 = half * 32; c0 < n_tile; c0 += 64) {
-        uint32_t r[32];
-        __syncwarp();
-        tmem_ld32(t_row + (uint32_t)c0, r);
-        const int nv = (n_tile - c0) < 32 ? (n_tile - c0) : 32;
-        const bool fast = fast_ok && nv == 32;
-        uint4 mk[4];
-        if (fast && ep.mask_src != nullptr) {    // in flight while the TMEM load completes
-          const uint4* mp = reinterpret_cast<const uint4*>(ep.mask_src + row * ep.ld_mask + n0 + c0);
-#pragma unroll
-          for (int g = 0; g < 4; ++g) mk[g] = __ldg(mp + g);
-        }
-        tmem_ld_wait();
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        // Full 32-column chunks leave through the TMA staging buffer; a partial chunk (tile width
-        // not a multiple of 32) is stored directly: its 32-wide box would spill into the
-        // neighbouring tile's columns (the tensor map clips only at the matrix edge).
-        const bool via_tma = (tma_p || tma_f) && nv == 32;
-        const bool st_f = !(tma_f && via_tma), st_p = !(tma_p && via_tma);
-        if (fast)
-          epilogue_fast(ep, v, row, n0 + c0, mk, st_f, st_p);
-        else
-          epilogue_chunk(ep, v, row, row_ok, n0 + c0, nv, lane,
-                         want_colsum ? s_colsum + q * kMaxBN + c0 : nullptr, st_f, st_p);
-        if (via_tma) {
-          if (lane == 0) bulk_wait_read0();      // the previous store has finished reading sbuf
-          __syncwarp();
-          if (tma_p)
-            stage_planes(sbuf, lane, v);
-          else
-            stage_f32(sbuf, lane, v);
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            if (tma_p) {
-              tma_store_2d(&tmO_hi, sbuf, n0 + c0, m0 + q * 32);
-              tma_store_2d(&tmO_lo, sbuf + 2048u, n0 + c0, m0 + q * 32);
-            } else {
-              tma_store_2d(&tmO_f32, sbuf, n0 + c0, m0 + q * 32);
-            }
-            bulk_commit();
-          }
-        }
-      }
-      if (ep.ones_col && ep.out_planes != nullptr && row_ok && half == 0 && n0 + n_tile == N) {
-        __nv_bfloat16* oh = ep.out_planes + row * 2 * ep.ldp + N;
-        oh[0] = __float2bfloat16_rn(1.f);
-        oh[ep.ldp] = __float2bfloat16_rn(0.f);
-      }
-      // accumulator drained -> the MMA warp may overwrite this stage
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(bar_tempty + 8u * acc, 0u);   // the leader's MMA warp waits on it
-      if (want_colsum) {
-        named_bar_sync(1, 32 * kEpiWarps);
-        const int t = threadIdx.x - 64;
-        for (int c = t; c < n_tile; c += 32 * kEpiWarps) {
-          const float s = ((s_colsum[c] + s_colsum[kMaxBN + c]) + s_colsum[2 * kMaxBN + c]) +
-                          s_colsum[3 * kMaxBN + c];
-          ep.colsum[(int64_t)m_blk * N + n0 + c] = s;
-        }
-        named_bar_sync(1, 32 * kEpiWarps);
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-    }
-    if ((tma_p || tma_f) && lane == 0) bulk_wait0();   // shared memory must outlive the stores
-  }
-  tc_fence_before();
-  cluster_sync();      // nobody leaves while the peer may still signal / read its shared memory
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, kTmemCols);
   }
 }
 
@@ -1027,23 +568,21 @@ struct DwDebug {
   uint32_t lbo_a, lbo_b, sbo;   // 0 = default
 };
 
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 tc_gemm_dw_kernel(const __grid_constant__ CUtensorMap tmA_hi,
                   const __grid_constant__ CUtensorMap tmA_lo,
                   const __grid_constant__ CUtensorMap tmG_hi,
-                  const __grid_constant__ CUtensorMap tmG_lo, int M, int Kin, int N, int BN,
-                  int stages, int rows_per_split, float* __restrict__ partials, DwDebug dbg) {
+                  const __grid_constant__ CUtensorMap tmG_lo, int M, int Kin, int N, int stages,
+                  int rows_per_split, float* __restrict__ partials, DwDebug dbg) {
+  constexpr int nb = BN / 64;                             // 64-column chunks of the G tile
+  constexpr uint32_t chunk = kDwBR * 128u;                // one TMA box: BR rows x 128 B
+  constexpr uint32_t a_bytes = 2u * chunk, b_bytes = (uint32_t)nb * chunk;
+  constexpr uint32_t stage_bytes = 2u * a_bytes + 2u * b_bytes;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* sm = smem_raw + (base - raw);
-  const int nb = (BN + 63) / 64;                         // 64-column chunks of the G tile
-  const uint32_t chunk = kDwBR * 128u;                   // one TMA box: BR rows x 128 B
-  const uint32_t a_bytes = 2u * chunk, b_bytes = (uint32_t)nb * chunk;
-  const uint32_t stage_bytes = 2u * a_bytes + 2u * b_bytes;
-  const uint32_t bar0 = base + (uint32_t)stages * stage_bytes;
-  const uint32_t bar_full = bar0, bar_empty = bar0 + 8u * stages, bar_tfull = bar0 + 16u * stages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + (size_t)stages * stage_bytes + 16 * stages + 32);
+  const uint32_t bar_full = base + (uint32_t)stages * stage_bytes, bar_empty = bar_full + 8u * stages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_n = (N + BN - 1) / BN;
@@ -1054,26 +593,18 @@ tc_gemm_dw_kernel(const __grid_constant__ CUtensorMap tmA_hi,
   r1 = r1 > M ? M : r1;
   const int nkb = r1 > r0 ? (r1 - r0 + kDwBR - 1) / kDwBR : 0;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmG_hi); prefetch_tmap(&tmG_lo);
     for (int s = 0; s < stages; ++s) {
       mbar_init(bar_full + 8u * s, 1);
-      mbar_init(bar_empty + 8u * s, 1);
+      mbar_init(bar_empty + 8u * s, kConsumerWarps);
     }
-    mbar_init(bar_tfull, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(smem_u32(tmem_slot), 256);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int kb = 0; kb < nkb; ++kb) {
@@ -1094,78 +625,57 @@ tc_gemm_dw_kernel(const __grid_constant__ CUtensorMap tmA_hi,
         if (++stage == stages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && nkb > 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int n_cur = N - n0;
-      n_cur = n_cur >= BN ? BN : ((n_cur + 15) & ~15);
-      const uint32_t idesc = umma_idesc(n_cur, 1, 1);
-      const uint32_t lbo_a = dbg.lbo_a ? dbg.lbo_a : chunk;
-      const uint32_t lbo_b = dbg.lbo_b ? dbg.lbo_b : chunk;
-      const uint32_t sbo = dbg.sbo ? dbg.sbo : 1024u;
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(bar_full + 8u * stage, phase, 0x600u + stage);
-        tc_fence_after();
-        const uint32_t sA = base + (uint32_t)stage * stage_bytes;
-        const uint32_t sB = sA + 2u * a_bytes;
-#pragma unroll
-        for (int j = 0; j < kDwBR / kUK; ++j) {
-          const uint32_t ko = (uint32_t)j * (kUK * 128u);  // 16 batch rows further down the box
-          const uint64_t a_hi = umma_desc(sA + ko, lbo_a, sbo);
-          const uint64_t a_lo = umma_desc(sA + a_bytes + ko, lbo_a, sbo);
-          const uint64_t g_hi = umma_desc(sB + ko, lbo_b, sbo);
-          const uint64_t g_lo = umma_desc(sB + b_bytes + ko, lbo_b, sbo);
-          tc_mma(tmem_base, a_hi, g_hi, idesc, (kb | j) != 0 ? 1u : 0u);
-          tc_mma(tmem_base, a_lo, g_hi, idesc, 1u);
-          tc_mma(tmem_base, a_hi, g_lo, idesc, 1u);
-        }
-        tc_commit(bar_empty + 8u * stage);
-        if (kb == nkb - 1) tc_commit(bar_tfull);
-        if (++stage == stages) { stage = 0; phase ^= 1u; }
-      }
-    }
   } else {
-    const int q = warp & 3;
-    const int krow = k0 + q * 32 + lane;
-    const int n_tile = (N - n0) < BN ? (N - n0) : BN;
-    float* out = partials + ((size_t)split * Kin + (size_t)krow) * N + n0;
-    const bool vec_ok = (reinterpret_cast<uintptr_t>(out) & 15u) == 0;
-    if (nkb > 0) {
-      mbar_wait(bar_tfull, 0, 0x700u);
-      tc_fence_after();
-    }
-    const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16);
-    for (int c0 = 0; c0 < n_tile; c0 += 32) {
-      uint32_t r[32];
-      if (nkb > 0) {
-        tmem_ld32(t_row + (uint32_t)c0, r);
-        tmem_ld_wait();
-      } else {
+    const int cw = warp - 4, wg = cw >> 2;
+    const uint32_t lbo_a = dbg.lbo_a ? dbg.lbo_a : chunk;
+    const uint32_t lbo_b = dbg.lbo_b ? dbg.lbo_b : chunk;
+    const uint32_t sbo = dbg.sbo ? dbg.sbo : 1024u;
+    float acc[BN / 2];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = 0u;
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kb = 0; kb < nkb; ++kb) {
+      mbar_wait(bar_full + 8u * stage, phase, 0x600u + stage);
+      // this warpgroup's 64 output rows (features k0 + 64 wg ..) are the wg-th column chunk of A
+      const uint32_t sA = base + (uint32_t)stage * stage_bytes + (uint32_t)wg * chunk;
+      const uint32_t sB = base + (uint32_t)stage * stage_bytes + 2u * a_bytes;
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < kDwBR / kUK; ++j) {
+        const uint32_t ko = (uint32_t)j * (kUK * 128u);  // 16 batch rows further down the box
+        const uint64_t a_hi = gmma_desc(sA + ko, lbo_a, sbo, 1u);
+        const uint64_t a_lo = gmma_desc(sA + a_bytes + ko, lbo_a, sbo, 1u);
+        const uint64_t g_hi = gmma_desc(sB + ko, lbo_b, sbo, 1u);
+        const uint64_t g_lo = gmma_desc(sB + b_bytes + ko, lbo_b, sbo, 1u);
+        Wgmma<BN, 1, 1>::mma(acc, a_hi, g_hi, 1u);
+        Wgmma<BN, 1, 1>::mma(acc, a_lo, g_hi, 1u);
+        Wgmma<BN, 1, 1>::mma(acc, a_hi, g_lo, 1u);
       }
-      if (krow < Kin) {
-        const int nv = (n_tile - c0) < 32 ? (n_tile - c0) : 32;
+      wgmma_commit();
+      if (kb > 0) {
+        wgmma_wait<1>();
+        if (lane == 0) mbar_arrive(bar_empty + 8u * prev);
+      }
+      prev = stage;
+      if (++stage == stages) { stage = 0; phase ^= 1u; }
+    }
+    wgmma_wait<0>();
+    fence_acc(acc);
+    const int kr0 = k0 + 64 * wg + 16 * (cw & 3) + (lane >> 2);
 #pragma unroll
-        for (int g = 0; g < 8; ++g) {
-          const int c = g * 4;
-          if (c + 4 <= nv && vec_ok) {
-            *reinterpret_cast<uint4*>(out + c0 + c) = make_uint4(r[c], r[c + 1], r[c + 2], r[c + 3]);
-          } else {
+    for (int j = 0; j < BN / 8; ++j) {
+      const int col = n0 + 8 * j + 2 * (lane & 3);
+      if (col >= N) continue;
+      const bool two = col + 1 < N;
 #pragma unroll
-            for (int j = 0; j < 4; ++j)
-              if (c + j < nv) out[c0 + c + j] = __uint_as_float(r[c + j]);
-          }
-        }
+      for (int h = 0; h < 2; ++h) {
+        const int krow = kr0 + 8 * h;
+        if (krow < Kin)
+          st_pair(partials + ((size_t)split * Kin + (size_t)krow) * N + col, two, acc[4 * j + 2 * h],
+                  acc[4 * j + 2 * h + 1]);
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
   }
 }
 
@@ -1266,32 +776,28 @@ static EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-// bf16 matrix [rows, width] with row pitch `pitch_elems`; box = box_w x box_rows, 128B swizzle,
-// out-of-bounds elements read as zero.
+// bf16 matrix [rows, width] with row pitch `pitch_elems`; box = box_w x box_rows, 128B swizzle
+// (64B for 32-wide boxes), out-of-bounds elements read as zero.
 static int make_map(CUtensorMap* m, const void* base, int64_t width, int64_t rows,
-                    int64_t pitch_elems, int box_w, int box_rows, int elem_bytes = 2) {
-  const CUtensorMapSwizzle swz = box_w * elem_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                                                           : CU_TENSOR_MAP_SWIZZLE_64B;
+                    int64_t pitch_elems, int box_w, int box_rows) {
+  const CUtensorMapSwizzle swz = box_w == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   EncodeTiledFn enc = encode_tiled_fn();
   if (enc == nullptr) {
     set_error("tc_gemm: cuTensorMapEncodeTiled is not available from this driver");
     return B200REC_ERR_CUDA;
   }
-  if ((reinterpret_cast<uintptr_t>(base) & 15u) != 0 || (pitch_elems * elem_bytes) % 16 != 0) {
+  if ((reinterpret_cast<uintptr_t>(base) & 15u) != 0 || (pitch_elems * 2) % 16 != 0) {
     set_error("tc_gemm: operand planes must be 16-byte aligned with a pitch multiple of 8 "
               "(base %p, pitch %lld)", base, (long long)pitch_elems);
     return B200REC_ERR_INVALID;
   }
   const cuuint64_t dims[2] = {(cuuint64_t)width, (cuuint64_t)rows};
-  const cuuint64_t strides[1] = {(cuuint64_t)pitch_elems * elem_bytes};
+  const cuuint64_t strides[1] = {(cuuint64_t)pitch_elems * 2};
   const cuuint32_t box[2] = {(cuuint32_t)box_w, (cuuint32_t)box_rows};
   const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = enc(m, elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                                            : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
-                         2, const_cast<void*>(base), dims,
+  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims,
                          strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("tc_gemm: cuTensorMapEncodeTiled failed (%d) width %lld rows %lld pitch %lld box %dx%d",
               (int)r, (long long)width, (long long)rows, (long long)pitch_elems, box_w, box_rows);
@@ -1300,20 +806,68 @@ static int make_map(CUtensorMap* m, const void* base, int64_t width, int64_t row
   return B200REC_OK;
 }
 
-static int pick_bn(int N) {
-  // <= 224 columns: two 128-byte-row stages + the output staging must fit 227 KB of shared memory
-  constexpr int kCap = 224;
-  const int tiles = (N + kCap - 1) / kCap;
-  int bn = (N + tiles - 1) / tiles;
-  bn = (bn + 15) & ~15;
-  return bn < 16 ? 16 : bn;
-}
-
 static DwDebug g_dw_debug = {0u, 0u, 0u};
 static int g_bn_override = 0;
-static int g_two_cta = 1;     // K-major GEMM on CTA pairs (cta_group::2) when M >= 4096 (0: never)
-static int g_tma_store = 1;   // epilogue outputs through TMA bulk stores (0: direct stores)
 static int g_bk = 64;   // k-block of the K-major kernel: 64 (SWIZZLE_128B) or 32 (SWIZZLE_64B)
+
+// Tile widths the K-major kernel is compiled for.  The choice minimises the padded output width
+// plus a per-tile charge of 64 columns for re-reading the A tile (N = 400 -> 2 x 208, 624 -> 3 x 208,
+// 1560 -> 8 x 208, 512 -> 2 x 256, 1 -> 16).  A forced width (tc_debug key 0) rounds up to the next
+// compiled one.
+static const int kTileBN[] = {16, 64, 128, 208, 256};
+
+static int pick_bn(int N) {
+  if (g_bn_override > 0) {
+    for (int bn : kTileBN)
+      if (bn >= g_bn_override) return bn;
+    return kMaxBN;
+  }
+  int best = kMaxBN;
+  int64_t best_cost = -1;
+  for (int bn : kTileBN) {
+    const int64_t cost = (int64_t)((N + bn - 1) / bn) * (bn + 64);
+    if (best_cost < 0 || cost <= best_cost) {
+      best = bn;
+      best_cost = cost;
+    }
+  }
+  return best;
+}
+
+template <int BN, int BK>
+static int launch_kmajor_tiles(const CUtensorMap (&mp)[4], int64_t M, int N, int K,
+                               const Epilogue& ep, cudaStream_t st) {
+  constexpr uint32_t stage_bytes = (2u * kBM + 2u * BN) * (uint32_t)BK * 2u;
+  constexpr uint32_t fixed = kConsumerWarps * kMaxBN * 4u + 16u * 8u + 1024u;
+  int stages = (int)((kSmemBudget - fixed) / stage_bytes);
+  stages = stages > 8 ? 8 : stages;
+  B200_REQUIRE(stages >= 2, "tc_gemm: tile does not fit shared memory");
+  const size_t smem = (size_t)stages * stage_bytes + 16 * stages + kConsumerWarps * kMaxBN * 4 + 1024;
+  static bool attr_set = false;
+  if (!attr_set) {
+    B200_CUDA(cudaFuncSetAttribute(tc_gemm_kmajor_kernel<BN, BK>,
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_set = true;
+  }
+  const int tiles = (int)((M + kBM - 1) / kBM) * ((N + BN - 1) / BN);
+  const int grid = tiles < sm_count() ? tiles : sm_count();
+  tc_gemm_kmajor_kernel<BN, BK><<<grid, kThreads, smem, st>>>(mp[0], mp[1], mp[2], mp[3], (int)M, N,
+                                                              K, stages, ep);
+  B200_LAUNCH_CHECK();
+  return B200REC_OK;
+}
+
+template <int BK>
+static int launch_kmajor_bk(int BN, const CUtensorMap (&mp)[4], int64_t M, int N, int K,
+                            const Epilogue& ep, cudaStream_t st) {
+  switch (BN) {
+    case 16: return launch_kmajor_tiles<16, BK>(mp, M, N, K, ep, st);
+    case 64: return launch_kmajor_tiles<64, BK>(mp, M, N, K, ep, st);
+    case 128: return launch_kmajor_tiles<128, BK>(mp, M, N, K, ep, st);
+    case 208: return launch_kmajor_tiles<208, BK>(mp, M, N, K, ep, st);
+    default: return launch_kmajor_tiles<256, BK>(mp, M, N, K, ep, st);
+  }
+}
 
 // D = A . B^T with A planes [M, 2*lda] (logical [M,K]) and B planes [N, 2*ldb] (logical [N,K]).
 static int launch_gemm_kmajor(const void* A, int64_t lda, const void* B, int64_t ldb, int64_t M,
@@ -1321,78 +875,18 @@ static int launch_gemm_kmajor(const void* A, int64_t lda, const void* B, int64_t
   B200_REQUIRE(M >= 0 && N > 0 && K > 0, "tc_gemm: bad sizes M=%lld N=%d K=%d", (long long)M, N, K);
   B200_REQUIRE(M < (1ll << 31), "tc_gemm: M too large");
   if (M == 0) return B200REC_OK;
-  const int BN = g_bn_override > 0 ? g_bn_override : pick_bn(N);
+  const int BN = pick_bn(N);
   const int BK = g_bk == 64 ? 64 : 32;
-  // CTA pairs pay off when there are enough 256-row tiles to fill the 74 clusters
-  const bool pair = g_two_cta != 0 && M >= 4096 && BN % 16 == 0 && ep.colsum == nullptr;
-  const uint32_t stage_bytes =
-      (2u * kBM + 2u * (uint32_t)(pair ? BN / 2 : BN)) * (uint32_t)BK * 2u;
-  const uint32_t staging_bytes = kEpiWarps * kStagingPerWarp;
-  int stages = (int)((kSmemBudget - 4096u - 16u * kMaxBN - staging_bytes) / stage_bytes);
-  stages = stages > 8 ? 8 : stages;
-  B200_REQUIRE(stages >= 2, "tc_gemm: tile does not fit shared memory");
-  const size_t smem =
-      (size_t)stages * stage_bytes + staging_bytes + 16 * stages + 64 + 16 * kMaxBN + 1024;
   const __nv_bfloat16* a = static_cast<const __nv_bfloat16*>(A);
   const __nv_bfloat16* b = static_cast<const __nv_bfloat16*>(B);
-  CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
+  CUtensorMap mp[4];
   int rc;
-  if ((rc = make_map(&ma_hi, a, K, M, 2 * lda, BK, kBM)) != B200REC_OK) return rc;
-  if ((rc = make_map(&ma_lo, a + lda, K, M, 2 * lda, BK, kBM)) != B200REC_OK) return rc;
-  const int b_rows = pair ? BN / 2 : BN;      // each CTA of a pair loads half of the B tile
-  if ((rc = make_map(&mb_hi, b, K, N, 2 * ldb, BK, b_rows)) != B200REC_OK) return rc;
-  if ((rc = make_map(&mb_lo, b + ldb, K, N, 2 * ldb, BK, b_rows)) != B200REC_OK) return rc;
-  // outputs through TMA stores where base and pitch allow it (else: direct stores from registers)
-  Epilogue e2 = ep;
-  CUtensorMap mo_hi = ma_hi, mo_lo = ma_hi, mo_f32 = ma_hi;   // placeholders when unused
-  e2.tma_planes = e2.tma_f32 = 0;
-  if (g_tma_store && ep.colsum == nullptr) {
-    if (ep.out_planes != nullptr && (reinterpret_cast<uintptr_t>(ep.out_planes) & 15u) == 0 &&
-        ep.ldp % 8 == 0) {
-      if ((rc = make_map(&mo_hi, ep.out_planes, N, M, 2 * ep.ldp, 32, 32)) != B200REC_OK) return rc;
-      if ((rc = make_map(&mo_lo, ep.out_planes + ep.ldp, N, M, 2 * ep.ldp, 32, 32)) != B200REC_OK)
-        return rc;
-      e2.tma_planes = 1;
-    } else if (ep.out_planes == nullptr && ep.out_f32 != nullptr &&
-               (reinterpret_cast<uintptr_t>(ep.out_f32) & 15u) == 0 && ep.ld_f32 % 4 == 0) {
-      if ((rc = make_map(&mo_f32, ep.out_f32, N, M, ep.ld_f32, 32, 32, 4)) != B200REC_OK) return rc;
-      e2.tma_f32 = 1;
-    }
-  }
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200_CUDA(cudaFuncSetAttribute(tc_gemm_kmajor_kernel<64>,
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    B200_CUDA(cudaFuncSetAttribute(tc_gemm_kmajor_kernel<32>,
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    B200_CUDA(cudaFuncSetAttribute(tc_gemm_kmajor2_kernel<64>,
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    B200_CUDA(cudaFuncSetAttribute(tc_gemm_kmajor2_kernel<32>,
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  if (pair) {
-    const int pair_tiles = (int)((M + 2 * kBM - 1) / (2 * kBM)) * ((N + BN - 1) / BN);
-    const int clusters = pair_tiles < sm_count() / 2 ? pair_tiles : sm_count() / 2;
-    if (BK == 64)
-      tc_gemm_kmajor2_kernel<64><<<2 * clusters, kThreadsK, smem, st>>>(
-          ma_hi, ma_lo, mb_hi, mb_lo, mo_hi, mo_lo, mo_f32, (int)M, N, K, BN, stages, e2);
-    else
-      tc_gemm_kmajor2_kernel<32><<<2 * clusters, kThreadsK, smem, st>>>(
-          ma_hi, ma_lo, mb_hi, mb_lo, mo_hi, mo_lo, mo_f32, (int)M, N, K, BN, stages, e2);
-    B200_LAUNCH_CHECK();
-    return B200REC_OK;
-  }
-  const int tiles = (int)((M + kBM - 1) / kBM) * ((N + BN - 1) / BN);
-  const int grid = tiles < sm_count() ? tiles : sm_count();
-  if (BK == 64)
-    tc_gemm_kmajor_kernel<64><<<grid, kThreadsK, smem, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, mo_hi, mo_lo,
-                                                             mo_f32, (int)M, N, K, BN, stages, e2);
-  else
-    tc_gemm_kmajor_kernel<32><<<grid, kThreadsK, smem, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, mo_hi, mo_lo,
-                                                             mo_f32, (int)M, N, K, BN, stages, e2);
-  B200_LAUNCH_CHECK();
-  return B200REC_OK;
+  if ((rc = make_map(&mp[0], a, K, M, 2 * lda, BK, kBM)) != B200REC_OK) return rc;
+  if ((rc = make_map(&mp[1], a + lda, K, M, 2 * lda, BK, kBM)) != B200REC_OK) return rc;
+  if ((rc = make_map(&mp[2], b, K, N, 2 * ldb, BK, BN)) != B200REC_OK) return rc;
+  if ((rc = make_map(&mp[3], b + ldb, K, N, 2 * ldb, BK, BN)) != B200REC_OK) return rc;
+  return BK == 64 ? launch_kmajor_bk<64>(BN, mp, M, N, K, ep, st)
+                  : launch_kmajor_bk<32>(BN, mp, M, N, K, ep, st);
 }
 
 struct DwPlan {
@@ -1402,7 +896,9 @@ struct DwPlan {
 
 static DwPlan plan_dw(int64_t M, int K, int N) {
   DwPlan p;
-  p.BN = g_bn_override > 0 ? g_bn_override : pick_bn(N);
+  // the G tile is loaded in 64-column chunks: widths 64, 128 or 256
+  p.BN = N <= 64 ? 64 : (N <= 128 ? 128 : 256);
+  if (g_bn_override > 0) p.BN = g_bn_override <= 64 ? 64 : (g_bn_override <= 128 ? 128 : 256);
   p.tiles = ((K + kBM - 1) / kBM) * ((N + p.BN - 1) / p.BN);
   int splits = sm_count() / p.tiles;
   splits = splits < 1 ? 1 : splits;
@@ -1412,13 +908,29 @@ static DwPlan plan_dw(int64_t M, int K, int N) {
   p.rows_per_split = (int)rps;
   p.splits = (int)((M + rps - 1) / rps);
   p.splits = p.splits < 1 ? 1 : p.splits;
-  const int nb = (p.BN + 63) / 64;
+  const int nb = p.BN / 64;
   const uint32_t stage_bytes = (4u + 2u * nb) * kDwBR * 128u;
   p.stages = (int)((kSmemBudget - 4096u) / stage_bytes);
   p.stages = p.stages > 8 ? 8 : p.stages;
-  p.smem = (size_t)p.stages * stage_bytes + 16 * p.stages + 64 + 1024;
+  p.smem = (size_t)p.stages * stage_bytes + 16 * p.stages + 1024;
   p.ws_bytes = (size_t)p.splits * K * N * sizeof(float);
   return p;
+}
+
+template <int BN>
+static int launch_dw_tiles(const DwPlan& p, const CUtensorMap (&mp)[4], int M, int K, int N,
+                           float* P, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    B200_CUDA(cudaFuncSetAttribute(tc_gemm_dw_kernel<BN>,
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_set = true;
+  }
+  dim3 grid(p.tiles, p.splits);
+  tc_gemm_dw_kernel<BN><<<grid, kThreads, p.smem, st>>>(mp[0], mp[1], mp[2], mp[3], M, K, N,
+                                                        p.stages, p.rows_per_split, P, g_dw_debug);
+  B200_LAUNCH_CHECK();
+  return B200REC_OK;
 }
 
 // dW[K,N] = A^T G with A planes [M, 2*lda] (logical [M,K]) and G planes [M, 2*ldg] (logical [M,N])
@@ -1438,23 +950,19 @@ static int launch_gemm_dw(const void* A, int64_t lda, const void* G, int64_t ldg
   }
   const __nv_bfloat16* a = static_cast<const __nv_bfloat16*>(A);
   const __nv_bfloat16* g = static_cast<const __nv_bfloat16*>(G);
-  CUtensorMap ma_hi, ma_lo, mg_hi, mg_lo;
+  CUtensorMap mp[4];
   int rc;
-  if ((rc = make_map(&ma_hi, a, K, M, 2 * lda, 64, kDwBR)) != B200REC_OK) return rc;
-  if ((rc = make_map(&ma_lo, a + lda, K, M, 2 * lda, 64, kDwBR)) != B200REC_OK) return rc;
-  if ((rc = make_map(&mg_hi, g, N, M, 2 * ldg, 64, kDwBR)) != B200REC_OK) return rc;
-  if ((rc = make_map(&mg_lo, g + ldg, N, M, 2 * ldg, 64, kDwBR)) != B200REC_OK) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200_CUDA(cudaFuncSetAttribute(tc_gemm_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   227 * 1024));
-    attr_set = true;
-  }
+  if ((rc = make_map(&mp[0], a, K, M, 2 * lda, 64, kDwBR)) != B200REC_OK) return rc;
+  if ((rc = make_map(&mp[1], a + lda, K, M, 2 * lda, 64, kDwBR)) != B200REC_OK) return rc;
+  if ((rc = make_map(&mp[2], g, N, M, 2 * ldg, 64, kDwBR)) != B200REC_OK) return rc;
+  if ((rc = make_map(&mp[3], g + ldg, N, M, 2 * ldg, 64, kDwBR)) != B200REC_OK) return rc;
   float* P = p.splits == 1 ? dW : static_cast<float*>(ws);
-  dim3 grid(p.tiles, p.splits);
-  tc_gemm_dw_kernel<<<grid, kThreads, p.smem, st>>>(ma_hi, ma_lo, mg_hi, mg_lo, (int)M, K, N, p.BN,
-                                                    p.stages, p.rows_per_split, P, g_dw_debug);
-  B200_LAUNCH_CHECK();
+  switch (p.BN) {
+    case 64: rc = launch_dw_tiles<64>(p, mp, (int)M, K, N, P, st); break;
+    case 128: rc = launch_dw_tiles<128>(p, mp, (int)M, K, N, P, st); break;
+    default: rc = launch_dw_tiles<256>(p, mp, (int)M, K, N, P, st); break;
+  }
+  if (rc != B200REC_OK) return rc;
   if (p.splits > 1) {
     const int64_t n4 = (KN + 3) / 4;
     tc_dw_reduce_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(P, p.splits, KN, dW);

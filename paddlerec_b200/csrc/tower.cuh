@@ -334,7 +334,7 @@ tower_head_bwd_kernel(const __nv_bfloat16* __restrict__ a, int64_t lda, int K,
   }
 }
 
-constexpr int kTowerRowSlices = 148 * 4;
+constexpr int kTowerRowSlices = 132 * 4;
 static int tower_row_slices(int64_t M) {
   return (int)min((int64_t)kTowerRowSlices, M > 0 ? M : (int64_t)1);
 }

@@ -108,7 +108,7 @@ class Linear(tnn.Module):
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if _PRECISION == "bf16x3" and x.is_cuda and ops.tc_backend():
-            return ops.tc_linear(x, self.weight, self.bias)      # hand-written tcgen05 GEMMs
+            return ops.tc_linear(x, self.weight, self.bias)      # hand-written wgmma GEMMs
         lead = x.shape[:-1]
         y = _LinearFn.apply(x.reshape(-1, self.in_features), self.weight, self.bias)
         return y.reshape(*lead, self.out_features)
@@ -234,12 +234,12 @@ class Embedding(tnn.Module):
 
 
 class FusedTable(tnn.Module):
-    """B200-native layout for a pair of tables that are always looked up with the same ids (DeepFM's
+    """Fused layout for a pair of tables that are always looked up with the same ids (DeepFM's
     second-order [V,D] and first-order [V,1], models/rank/deepfm/net.py:66-86): ONE array of
     128-byte slots `[D emb | w1 | pad]`.
 
-    Why: on B200 a random 64-byte row costs a full 128-byte DRAM access and so does a random 4-byte
-    scalar (profiles/r1_gather_variants_microbench.txt), so the reference's two-table layout moves
+    Why: a random 64-byte row costs a full 128-byte DRAM access and so does a random 4-byte
+    scalar (tools/microbench/gather_variants.cu measures it), so the reference's two-table layout moves
     256 B per looked-up id for 68 useful bytes; the slot moves 128 B.  Same for the optimizer.
 
     state_dict() still exposes the reference's two keys (`embedding.weight` [V,D] and

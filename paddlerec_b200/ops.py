@@ -526,7 +526,7 @@ def raw_shard_push_rows(rows: torch.Tensor, D: int, seg_dev: torch.Tensor, dst_d
     _count("shard_push_rows")
 
 
-# ---- tcgen05 tower GEMMs (csrc/tc_gemm.cuh) ---------------------------------------------------
+# ---- wgmma tower GEMMs (csrc/tc_gemm.cuh) ---------------------------------------------------
 def plane_ld(n: int, ones_col: bool = False) -> int:
     """Plane pitch of a logical width n (+1 with a ones column): the hi and lo planes must both be
     16-byte aligned."""
@@ -584,7 +584,7 @@ def raw_tc_prep_weight(W: torch.Tensor, want_w: bool = True, want_wt: bool = Tru
 
 def raw_tc_linear_fwd(a_planes: torch.Tensor, K: int, WTp: torch.Tensor, N: int, bias, relu: bool,
                       want_f32: bool, want_planes: bool, ones_col: bool = False):
-    """y = a @ W + bias (ReLU optional) on the tcgen05 tensor cores.  Returns (y fp32 [M,N] | None,
+    """y = a @ W + bias (ReLU optional) on the wgmma tensor cores.  Returns (y fp32 [M,N] | None,
     planes(y) [M, 2*ld] | None)."""
     lib = _lib.load()
     M = a_planes.shape[0]
@@ -603,7 +603,7 @@ def raw_tc_linear_fwd(a_planes: torch.Tensor, K: int, WTp: torch.Tensor, N: int,
 def raw_tc_cross_fwd(xl_planes, WTp, bias, x0, xl, want_planes: bool, want_u: bool = False,
                      ones_col: bool = False):
     """CrossNetV2 layer out = x0 * u + xl, u = xl @ W + b, with the Hadamard/residual epilogue fused
-    into the tcgen05 GEMM.  Returns (out fp32 [M,C], planes(out) | None, u fp32 | None)."""
+    into the wgmma GEMM.  Returns (out fp32 [M,C], planes(out) | None, u fp32 | None)."""
     lib = _lib.load()
     x0 = _req(x0, torch.float32, "x0")
     xl = _req(xl, torch.float32, "xl")
@@ -652,7 +652,7 @@ def raw_tc_linear_bwd_dx(g_planes, N: int, Wp, K: int, mask_planes, want_f32: bo
 
 def raw_tc_linear_bwd_dw(a_planes, K: int, g_planes, N: int, bias_row: bool = False,
                          ws_tag: str = "tc_bwd"):
-    """dW [K,N] = a^T @ g (batch-split tcgen05 GEMM + fixed-order reduce).  With bias_row the
+    """dW [K,N] = a^T @ g (batch-split wgmma GEMM + fixed-order reduce).  With bias_row the
     operand `a` carries a column of ones at index K (ones_col of raw_tc_split / raw_tc_linear_fwd)
     and the result is (dW [K,N], dbias [N]) — the bias gradient is row K of the same GEMM."""
     lib = _lib.load()
@@ -801,13 +801,13 @@ def raw_auc_update(pred: torch.Tensor, label: torch.Tensor, stat_pos: torch.Tens
 
 
 def tc_debug(key: int, value: int) -> None:
-    """Bring-up / tuning knobs of the tcgen05 GEMMs (0: force tile width BN; 0 = automatic)."""
+    """Bring-up / tuning knobs of the wgmma GEMMs (0: force tile width BN; 0 = automatic)."""
     lib = _lib.load()
     check(lib.b200rec_tc_debug(key, value), "tc_debug")
 
 
 def tc_timeout_word() -> int:
-    """Non-zero if a pipeline watchdog of the tcgen05 kernels fired (which wait, see tc_gemm.cuh)."""
+    """Non-zero if a pipeline watchdog of the wgmma kernels fired (which wait, see tc_gemm.cuh)."""
     lib = _lib.load()
     w = ctypes.c_uint(0)
     check(lib.b200rec_tc_timeout_word(ctypes.byref(w)), "tc_timeout_word")
@@ -926,13 +926,13 @@ def gather_pool_sum(W, keys, offsets, padding_idx, sink, hook):
 
 
 def tc_backend() -> bool:
-    """True when the hand-written tcgen05 GEMMs serve the 'bf16x3' matmuls (tower.BACKEND)."""
+    """True when the hand-written wgmma GEMMs serve the 'bf16x3' matmuls (tower.BACKEND)."""
     from . import tower
     return tower.BACKEND == "tcgen05"
 
 
 class _TcLinear(torch.autograd.Function):
-    """y = x @ W (+ b) as ONE tcgen05 GEMM per direction (split precision): forward with the bias in
+    """y = x @ W (+ b) as ONE wgmma GEMM per direction (split precision): forward with the bias in
     the epilogue, dW as the batch-split MN-major GEMM (the bias gradient rides along as an extra
     output row when the input width is not a multiple of 128), dx as the K-major GEMM.  Used by
     every nn.Linear / split_mm of the package in 'bf16x3' precision."""
@@ -969,7 +969,7 @@ def tc_linear(x, W, b=None):
 
 
 class _CrossV2Tc(torch.autograd.Function):
-    """One CrossNetV2 layer X_{i+1} = X_i + X_0 * (X_i W + b) (dcn_v2/net.py:222-226) on the tcgen05
+    """One CrossNetV2 layer X_{i+1} = X_i + X_0 * (X_i W + b) (dcn_v2/net.py:222-226) on the wgmma
     kernels: ONE GEMM whose epilogue applies bias, Hadamard and residual, saves u = X_i W + b for
     the backward and emits the next layer's hi/lo operand; backward = K3 (dxw, dx0) + the split +
     the dW GEMM + the dX GEMM with the residual gradient added in its epilogue."""
@@ -1388,7 +1388,7 @@ def gather(W, ids, padding_idx, sink, hook):
 
 def cross_v2(x0, xl, W, bias, mm, precision="fp32", xl_planes=None):
     """-> (X_{i+1}, its hi/lo planes or None).  Pass the planes back as `xl_planes` of the next
-    layer: on the tcgen05 back end the GEMM epilogue has already produced that operand."""
+    layer: on the wgmma back end the GEMM epilogue has already produced that operand."""
     if precision == "bf16x3" and x0.is_cuda and tc_backend():
         return _CrossV2Tc.apply(x0, xl, W, bias, xl_planes)
     return _CrossV2.apply(x0, xl, W, bias, mm, precision), None

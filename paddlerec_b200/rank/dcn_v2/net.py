@@ -3,9 +3,9 @@ models/rank/dcn_v2/net.py (DCN_V2Layer :21-137, DNNLayer :140-184, DeepCrossLaye
 CrossNetV2 :214-226, CrossNetMix :229-320).
 
 CUDA path: the 26-slot lookup is b200rec_gather (+ sorted segment-reduce backward); every
-CrossNetV2 layer is ONE hand-written tcgen05 GEMM whose epilogue applies bias, Hadamard and residual
-and emits the next layer's operand (ops._CrossV2Tc); the MLP is the tcgen05 tower (tower.py) in
-eval mode and per-layer tcgen05 Linears around the reference's dropouts in train mode.  CrossNetMix is re-associated from the reference's per-sample
+CrossNetV2 layer is ONE hand-written wgmma GEMM whose epilogue applies bias, Hadamard and residual
+and emits the next layer's operand (ops._CrossV2Tc); the MLP is the wgmma tower (tower.py) in
+eval mode and per-layer wgmma Linears around the reference's dropouts in train mode.  CrossNetMix is re-associated from the reference's per-sample
 [B,in,1] batched GEMVs into three batched GEMMs over all experts (mathematically identical).
 Quirks kept (SURVEY.md Q5, Q10, Q13): Dropout(0.5) after every Linear AND every ReLU in train
 mode; L2Decay(1e-7) on the DNN weights (applied by the optimizer, optim._apply_regularizers); dense_emb is a full Linear(13 -> 13*D).

@@ -1,6 +1,6 @@
 """DeepFM network — same classes, constructor arguments, forward signature and state_dict names as
 the reference's models/rank/deepfm/net.py (DeepFMLayer :21-49, FM :52-139, DNN :142-174), with the
-FM body replaced by ONE fused sm_100a kernel (b200rec_embed_fm_fwd / _bwd).
+FM body replaced by ONE fused sm_90a kernel (b200rec_embed_fm_fwd / _bwd).
 
 Reference quirks kept on purpose (SURVEY.md Appendix C): `self.bias` exists but is never added to
 the logit (Q1); both tables use padding_idx=0 (row 0 reads as zeros and gets no gradient).

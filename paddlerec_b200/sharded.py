@@ -101,10 +101,9 @@ FUSED_PUSH = os.environ.get("B200REC_FUSED_PUSH", "0") == "1"
 def p2p_enabled(world: int) -> bool:
     """Peer-memory exchange on/off.  B200REC_P2P=1 forces it on, =0 off; unset = on for up to
     P2P_MAX_WORLD ranks.  The limit is the largest world size the peer-memory path has completed
-    tests + bench on (2 and 4 ranks, profiles/r2g_*, r2h_*, r2j_*); the one 8-rank bench attempt with
-    it did not finish inside its 300 s limit and could not be diagnosed (DESIGN.md section 5), so
-    more than 4 ranks use the NCCL all-to-all exchange, which is validated at 8
-    (profiles/r2_sharded_parity_n8.log, profiles/r2k_cfg3_dcn_n8.jsonl)."""
+    tests + bench on (2 and 4 ranks); the one 8-rank bench attempt with it did not finish and could
+    not be diagnosed (DESIGN.md section 5), so more than 4 ranks use the NCCL all-to-all exchange,
+    which the sharded parity tests have run at 8 ranks."""
     env = os.environ.get("B200REC_P2P", "auto")
     if env == "0":
         return False

@@ -15,7 +15,7 @@ consumes), never as fp32.
                         dx = [dz_hi|dz_lo] @ [W_hi|W_hi]^T (+)= dz_hi @ W_lo^T   2 GEMMs
 
 Two back ends with the same arithmetic (three bf16 products per fp32 product, fp32 accumulation):
-  'tcgen05' (default)  hand-written tcgen05.mma / TMEM / TMA GEMMs (csrc/tc_gemm.cuh) whose
+  'tcgen05' (default; the name predates the Hopper port)  hand-written wgmma / TMA GEMMs (csrc/tc_gemm.cuh) whose
                        epilogues apply bias + ReLU and emit the NEXT layer's hi/lo operand directly
                        (forward), or the ReLU mask + split + bias column-sum (backward); dW is a
                        batch-split GEMM on MN-major operands.  No elementwise kernel runs between
@@ -70,12 +70,12 @@ def _side_stream(device) -> "torch.cuda.Stream":
 def set_backend(name: str) -> None:
     global BACKEND
     if name not in ("tcgen05", "cublas"):
-        raise ValueError("tower backend must be tcgen05 or cublas")
+        raise ValueError("tower backend must be wgmma or cublas")
     BACKEND = name
 
 
 class _TowerTcFn(torch.autograd.Function):
-    """The whole Linear/ReLU chain on the tcgen05 kernels.  Saved for backward: the split
+    """The whole Linear/ReLU chain on the wgmma kernels.  Saved for backward: the split
     activations of every layer (they are the dW operands and the ReLU masks) and planes(W)."""
 
     @staticmethod

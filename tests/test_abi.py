@@ -1,4 +1,4 @@
-"""The drop-in boundary: libb200rec.so builds for sm_100a, loads, and exports every symbol that
+"""The drop-in boundary: libb200rec.so builds for sm_90a, loads, and exports every symbol that
 include/b200rec.h declares.  No compute calls (runs without a GPU)."""
 import ctypes
 import os
@@ -26,12 +26,12 @@ def test_every_declared_symbol_is_exported_and_bound():
     assert set(_lib._SIG) == set(declared)
 
 
-def test_binary_targets_sm_100a_only():
+def test_binary_targets_sm_90a_only():
     out = subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True)
     if out.returncode != 0:
         pytest.skip("cuobjdump unavailable")
-    assert "sm_100a" in out.stdout
-    assert "sm_90" not in out.stdout and "sm_80" not in out.stdout
+    assert "sm_90a" in out.stdout
+    assert "sm_100" not in out.stdout and "sm_80" not in out.stdout
 
 
 def test_no_cpu_fallback_on_cpu_tensors():

@@ -6,6 +6,7 @@ unmodified) — see tests/golden/make_reader_golden.py.  Integer output (ids, la
 be bit-exact; float32 dense values bit-exact against the Python reader, and within the 6
 significant digits parser.cpp prints against its text output.
 """
+import gzip
 import os
 import subprocess
 
@@ -108,9 +109,10 @@ def test_criteo_tsv_matches_golden_from_reference_parser_cpp():
     assert np.array_equal(od, dense)                          # bit-exact vs the restatement
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(ROOT, "oracle", "_ref", "criteo_parser")),
-                    reason="oracle/_ref/criteo_parser not built (needs /root/reference)")
 def test_criteo_tsv_matches_reference_binary_live():
+    """700 random lines (empty fields, negative dense values, 40-bit hex ids) against what the
+    reference's parser.cpp printed for them (tests/golden/criteo_tsv_parser_cpp_random.txt.gz); where
+    oracle/_ref/criteo_parser has been built, its live output must still be exactly that."""
     rng = np.random.default_rng(5)
     lines = []
     for _ in range(700):
@@ -119,8 +121,10 @@ def test_criteo_tsv_matches_reference_binary_live():
         cols += ["" if rng.random() < 0.2 else "%x" % rng.integers(0, 1 << 40) for _ in range(26)]
         lines.append("\t".join(cols))
     tsv = ("\n".join(lines) + "\n").encode()
-    out = subprocess.run([os.path.join(ROOT, "oracle", "_ref", "criteo_parser")], input=tsv,
-                         capture_output=True, check=True).stdout
+    out = gzip.decompress(_read("criteo_tsv_parser_cpp_random.txt.gz"))
+    exe = os.path.join(ROOT, "oracle", "_ref", "criteo_parser")
+    if os.path.exists(exe):
+        assert subprocess.run([exe], input=tsv, capture_output=True, check=True).stdout == out
     rl, rid, rd = _parser_cpp_output(out)
     for threads in (1, 3):
         label, ids, dense, skipped = dataio.parse_criteo_tsv(tsv, threads=threads)

@@ -340,7 +340,7 @@ def test_tower_mlp_matches_fp64(last_act):
 
 @pytest.mark.parametrize("D", [4, 9, 16])
 def test_fused_slot_layout_equals_two_tables(D):
-    """The B200-native fused slot layout ([D emb | w1 | pad] per 128-byte row) must give exactly the
+    """The fused slot layout ([D emb | w1 | pad] per 128-byte row) must give exactly the
     same forward and the same gradients as the reference's two-table layout."""
     ops = _ops()
     B, F, Dn, V = 65, 26, 13, 300

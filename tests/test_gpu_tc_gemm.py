@@ -1,4 +1,4 @@
-"""tcgen05 / TMEM / TMA tower GEMMs (csrc/tc_gemm.cuh) through the C ABI vs an fp64 product of the
+"""wgmma / TMA tower GEMMs (csrc/tc_gemm.cuh) through the C ABI vs an fp64 product of the
 same fp32 operands.  Split precision (bf16x3) drops only the lo*lo term and the residual of the
 residual: ~2^-17 per product, so 5e-5 of the output's max-norm is a tight bar (TF32 would be 5e-4).
 Edge cases: M, N, K not multiples of the tile (128 x BN x 64), N = 1, K = 1, forced narrow tiles,
@@ -61,7 +61,8 @@ def test_tc_linear_fwd(M, N, K, relu):
 @pytest.mark.parametrize("bn", [16, 64, 128, 224])
 @pytest.mark.parametrize("bk", [32, 64])
 def test_tc_linear_fwd_tile_shapes(bn, bk):
-    """Forced tile widths and both k-block / swizzle variants (64 B and 128 B rows)."""
+    """Forced tile widths (rounded up to a compiled one: 16, 64, 128, 256) and both k-block / swizzle
+    variants (64 B and 128 B rows); the three calls emit fp32 only, planes only and both."""
     ops = _ops()
     g = torch.Generator().manual_seed(bn)
     M, N, K = 700, 400, 624
@@ -74,13 +75,11 @@ def test_tc_linear_fwd_tile_shapes(bn, bk):
     try:
         y, _ = ops.raw_tc_linear_fwd(a, K, WTp, N, None, False, True, False)
         _, yp = ops.raw_tc_linear_fwd(a, K, WTp, N, None, False, False, True)
-        ops.tc_debug(5, 0)      # direct register stores instead of TMA bulk stores
         y2, yp2 = ops.raw_tc_linear_fwd(a, K, WTp, N, None, False, True, True)
         torch.cuda.synchronize()
     finally:
         ops.tc_debug(0, 0)
         ops.tc_debug(4, 64)
-        ops.tc_debug(5, 1)
     want = x.double() @ W.double()
     assert _err(y, want) < 5e-5 and _err(_join(yp, N), want) < 5e-5
     assert torch.equal(y, y2) and torch.equal(yp[:, :N], yp2[:, :N])
@@ -153,13 +152,13 @@ def test_tc_linear_bwd_dw(M, K, N):
     assert torch.equal(dW, dW2)
 
 
-@pytest.mark.parametrize("pair", [0, 1])
-def test_tc_many_tiles_per_cta(pair):
-    """More output tiles than SMs: every CTA walks several tiles, alternating the two TMEM
-    accumulator stages while the epilogue of the previous tile is still draining; rows 39936..
-    exercise the partially valid last row block."""
+@pytest.mark.parametrize("bk", [32, 64])
+def test_tc_many_tiles_per_cta(bk):
+    """More output tiles than SMs: every CTA walks several tiles while the producer already streams
+    the next tile's k-blocks into the pipeline stages the epilogue of the previous one has freed;
+    rows 39936.. exercise the partially valid last row block.  Both k-block widths (pipeline depths)."""
     ops = _ops()
-    ops.tc_debug(6, pair)
+    ops.tc_debug(4, bk)
     g_ = torch.Generator().manual_seed(77)
     M, K, N = 40003, 400, 64
     x = torch.randn(M, N, generator=g_)
@@ -185,7 +184,7 @@ def test_tc_many_tiles_per_cta(pair):
     torch.cuda.synchronize()
     wantdx = (wantg @ W2.double().t()) * (act.double() > 0)
     assert _err(dx, wantdx) < 5e-5 and _err(_join(dxp, N), wantdx) < 5e-5
-    ops.tc_debug(6, 1)
+    ops.tc_debug(4, 64)
     # element-wise on the tail rows (a max-norm bound would hide one bad row)
     assert _err(dx[-80:], wantdx[-80:]) < 5e-5
 
@@ -212,7 +211,7 @@ def test_tc_cross_fwd():
 
 
 def test_cross_v2_layer_chain_autograd():
-    """Two chained CrossNetV2 layers through ops.cross_v2 on the tcgen05 back end (the second
+    """Two chained CrossNetV2 layers through ops.cross_v2 on the wgmma back end (the second
     consumes the planes the first one's epilogue emitted): output and every gradient vs fp64."""
     from paddlerec_b200 import nn as bnn
     from tests.util import rel_err
@@ -347,9 +346,9 @@ def test_tc_head_width1_layer(M, K):
 
 
 @pytest.mark.parametrize("M,N,K", [(20000, 400, 624), (4099, 624, 400), (8192, 40, 1560)])
-def test_tc_cta_pair_kernel(M, N, K):
-    """The cta_group::2 variant (two SMs per 256-row tile, B split across the pair, multicast
-    commits, remote barrier arrivals): forward with every output kind, masked dX, odd tile counts."""
+def test_tc_large_m_every_output_kind(M, N, K):
+    """Tower-sized row counts with several tiles per CTA: forward with every output kind, masked
+    dX, odd tile counts."""
     ops = _ops()
     g = torch.Generator().manual_seed(M + N)
     x = torch.randn(M, K, generator=g)
@@ -358,17 +357,13 @@ def test_tc_cta_pair_kernel(M, N, K):
     a = ops.raw_tc_split(x.to(DEV))
     Wp, WTp = ops.raw_tc_prep_weight(W.to(DEV))
     want = (x.double() @ W.double() + b.double()).clamp_min(0)
-    ops.tc_debug(6, 1)
-    try:
-        y, _ = ops.raw_tc_linear_fwd(a, K, WTp, N, b.to(DEV), True, True, False)
-        _, yp = ops.raw_tc_linear_fwd(a, K, WTp, N, b.to(DEV), True, False, True, ones_col=True)
-        gy = torch.randn(M, N, generator=g)
-        gp, _ = ops.raw_tc_split_bwd(gy.to(DEV), None)
-        dx, _, _ = ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, None, True, False, False)
-        _, dxp, _ = ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, a, False, True, False)
-        torch.cuda.synchronize()
-    finally:
-        ops.tc_debug(6, 1)
+    y, _ = ops.raw_tc_linear_fwd(a, K, WTp, N, b.to(DEV), True, True, False)
+    _, yp = ops.raw_tc_linear_fwd(a, K, WTp, N, b.to(DEV), True, False, True, ones_col=True)
+    gy = torch.randn(M, N, generator=g)
+    gp, _ = ops.raw_tc_split_bwd(gy.to(DEV), None)
+    dx, _, _ = ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, None, True, False, False)
+    _, dxp, _ = ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, a, False, True, False)
+    torch.cuda.synchronize()
     assert _err(y, want) < 5e-5 and _err(_join(yp, N), want) < 5e-5
     wdx = gy.double() @ W.double().t()
     assert _err(dx, wdx) < 5e-5

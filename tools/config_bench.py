@@ -5,7 +5,7 @@
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \\
         --master-port 29511 tools/config_bench.py --what dcn
 
-  dcn     config 3: DCN-V2 Criteo-shape (D=40, CrossNetV2 x2 on the tcgen05 kernels, fc [768,768],
+  dcn     config 3: DCN-V2 Criteo-shape (D=40, CrossNetV2 x2 on the wgmma kernels, fc [768,768],
           Adam + global-norm clip), embedding table row-sharded (id mod N) with the NCCL all-to-all
           exchange, dense parameters data-parallel; weak scaling, B per GPU fixed.
   din     config 4: DIN AmazonElec-shape (63001 items / 801 cats, E=64+64, history 100): tables are
@@ -167,7 +167,7 @@ def run_din(a, rank, world, dev):
     ms = timed(step, a.iters, 2, world, dev)
     flop = 3 * 2.0 * B * L * (2 * 128 * 80 + 80 * 40 + 40)
     emit(rank, {"config": 4, "what": "DIN AmazonElec-shape train step (7 gathers, fused attention "
-                "fwd + bwd, output MLP on the tcgen05 Linears, SGD)", "n_gpus": world, "B_per_gpu": B,
+                "fwd + bwd, output MLP on the wgmma Linears, SGD)", "n_gpus": world, "B_per_gpu": B,
                 "L": L, "ms_per_step": ms, "samples_per_s": B * world / ms * 1e3, "scaling": "weak",
                 "parallelism": "replicas only (tables are 63001 x 64: nothing to shard, no collective)",
                 "attention_tflops_fp32_lower_bound": round(flop / (ms / 1e3) / 1e12, 2)})

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """K6 (DLRM dot interaction) and the feasign fold, timed alone: CUDA events around `iters` launches
-after warm-up, over a ring of inputs larger than L2 (126 MB) so every launch reads from HBM.
+after warm-up, over a ring of inputs larger than L2 (50 MB) so every launch reads from HBM.
 Reports algorithmic GB/s: forward 4*(N*d + d + P) B/sample, backward 4*(2*N*d + d + P),
 hash_keys 16 (+4 with slots) B/key; the library formulation (bmm + triu gather + cat) beside it."""
 import argparse

@@ -12,7 +12,7 @@ timeout 200 python tools/tc_probe.py perf > $O/${P}_tc_perf.jsonl 2>&1
 if [ "$M" = "final" ]; then
   timeout 500 python bench.py --steps 20 --warmup 5 2>&1 | tail -1 > $O/${P}_bench_n1.json
   timeout 300 python bench.py --impl reference --steps 4 --warmup 1 2>&1 | tail -1 > $O/${P}_bench_reference_arm.json
-  # compute-sanitizer on the smoke step (K1, K2, tcgen05 tower at a small size, lazy Adam)
+  # compute-sanitizer on the smoke step (K1, K2, wgmma tower at a small size, lazy Adam)
   timeout 300 compute-sanitizer --tool memcheck --error-exitcode 9 python -c "import __graft_entry__ as g; g.smoke()" > $O/${P}_sanitizer_memcheck.log 2>&1; echo "memcheck rc=$?" >> $O/${P}_sanitizer_memcheck.log
   B200REC_TEST_EXPERIMENTAL=1 timeout 200 python -m pytest tests/test_gpu_kernels.py -q -k "v2" -rf 2>&1 | tail -5 > $O/${P}_k6_v2.log
   # opt-in paths that have not run on a GPU yet (ahead-of-time grouping; fused push needs >= 2 GPUs)

@@ -3,7 +3,7 @@
 
     python tools/kernel_sweep.py [--quick]
 Prints one JSON line per (kernel, V, D, distribution): time, algorithmic GB/s, fraction of the
-measured HBM peak.  Used to fill DESIGN.md / profiles/ and BASELINE config 5 (W&D gather sweep).
+measured HBM peak.  Used for BASELINE config 5 (W&D gather sweep).
 """
 import argparse
 import json
@@ -71,7 +71,7 @@ def main():
                 alg = B * (F * 8 + Dn * 4 + F * 4 * D + F * 4 + (F + Dn) * 4 * D + 8)
                 print(json.dumps({"kernel": "embed_fm_fwd", "V": V, "D": D, "dist": dist, "ms": ms,
                                   "GBps": alg / ms / 1e6, "frac": alg / ms / 1e6 / PEAK}), flush=True)
-                if D + 1 <= 32:   # B200-native fused slot layout [D emb | w1 | pad] (128-byte rows)
+                if D + 1 <= 32:   # fused slot layout [D emb | w1 | pad] (128-byte rows)
                     Wf = torch.zeros(V, 32, device=dev)
                     Wf[:, :D] = W
                     Wf[:, D] = W1[:, 0]

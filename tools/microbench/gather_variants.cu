@@ -1,6 +1,6 @@
-// Micro-benchmark: how should 64-byte random rows be fetched on B200?
+// Micro-benchmark: how should 64-byte random rows be fetched on the H100?
 // Variants of the load instruction x cudaLimitMaxL2FetchGranularity, timed with CUDA events.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gather_variants gather_variants.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o gather_variants gather_variants.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

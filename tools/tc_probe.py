@@ -1,4 +1,4 @@
-"""Bring-up probe for the tcgen05 GEMMs: every stage runs in its own process (a pipeline watchdog
+"""Bring-up probe for the wgmma GEMMs: every stage runs in its own process (a pipeline watchdog
 trap kills the CUDA context), prints max relative error vs fp64 and kernel time.
 
     python tools/tc_probe.py            # all stages
@@ -95,11 +95,9 @@ def stage(name, arg):
             fl = 3 * 2.0 * M * K * N
             for bn in ([0] if not arg else [int(v) for v in arg.split(",")]):
                 ops.tc_debug(0, bn)
-                for bk, tma, pair in ((64, 1, 0), (64, 1, 1), (32, 1, 1), (64, 0, 0)):
+                for bk in (64, 32):
                     ops.tc_debug(4, bk)
-                    ops.tc_debug(5, tma)
-                    ops.tc_debug(6, pair)
-                    tag = "%dx%d bn%d bk%d tma%d pair%d" % (K, N, bn, bk, tma, pair)
+                    tag = "%dx%d bn%d bk%d" % (K, N, bn, bk)
                     t = _time(lambda: ops.raw_tc_linear_fwd(a, K, WTp, N, b, True, False, True))
                     res["fwd " + tag] = [round(t, 4), round(fl / t / 1e9, 1)]
                     t = _time(lambda: ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, a, False, True, False))
@@ -109,8 +107,6 @@ def stage(name, arg):
                     t = _time(lambda: ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, None, True, False, False))
                     res["dx f32 " + tag] = [round(t, 4), round(fl / t / 1e9, 1)]
                 ops.tc_debug(4, 64)
-                ops.tc_debug(5, 1)
-                ops.tc_debug(6, 1)
                 t = _time(lambda: ops.raw_tc_linear_bwd_dw(a, K, gp, N))
                 res["dw  %dx%d bn%d" % (K, N, bn)] = [round(t, 4), round(fl / t / 1e9, 1)]
             ops.tc_debug(0, 0)
