@@ -256,10 +256,10 @@ def dot_interact(T, self_interaction: bool = False):
     because triu(Z, 1) has already zeroed them (:105-113); R = concat([x, Zflat]) (:115)."""
     B, N, d = T.shape
     Z = torch.bmm(T, T.transpose(1, 2))
-    iu = torch.triu_indices(N, N, 0 if self_interaction else 1)
+    iu = torch.triu_indices(N, N, 0 if self_interaction else 1, device=T.device)
     flat = Z[:, iu[0], iu[1]]
     if self_interaction:
-        flat = torch.where((iu[0] == iu[1]).unsqueeze(0), torch.zeros((), dtype=T.dtype), flat)
+        flat = torch.where((iu[0] == iu[1]).unsqueeze(0), torch.zeros((), dtype=T.dtype, device=T.device), flat)
     return torch.cat([T[:, N - 1, :], flat], 1)
 
 

@@ -1,0 +1,887 @@
+"""Persistent and grid-stride kernels at sizes where every CTA (or warp, or lane group) loops.
+
+The unit tests in test_gpu_kernels.py run these kernels where the grid is not yet capped, so each
+CTA makes one pass or none.  Here every size is computed from the launcher's grid formula and the
+device's SM count (the library reads the same attribute, b200rec.cu:32-43), and each test asserts
+that every CTA / warp / lane group makes at least MIN_ITERS passes of its loop.  The C++ constants
+are mirrored below with the line that defines them: if one changes, the iteration assertions fail
+instead of the test silently shrinking back into the one-pass regime.
+
+Every value is compared ELEMENT-WISE with a float64 reference of the same operation computed on the
+GPU.  fp32 sums are held to
+    |got - want| <= k * 2^-24 * sum|terms|        (per element)
+where k is the longest chain of fp32 roundings the kernel's summation order can put on that
+element; each test's docstring derives its k from the kernel's loop structure.  Copies, gathers and
+single correctly-rounded products are compared with torch.equal, and the paths documented as
+fixed-order are run twice and must be bit-identical.
+"""
+import math
+import os
+
+import numpy as np
+import pytest
+import torch
+
+from oracle import nets
+from oracle import optim as ooptim
+
+pytestmark = pytest.mark.gpu
+
+DEV = "cuda"
+U = 2.0 ** -24            # unit roundoff of fp32
+MIN_ITERS = 3
+
+# ---- C++ constants mirrored here (file:line of the definition) ---------------------------------
+DIN_TILE = 64             # din_attn.cuh:28   kDinTile; grid = min(tiles, SM) din_attn.cuh:627-630,693-694
+DIN_H1, DIN_H2 = 80, 40   # din_attn.cuh:26-27
+SEG_THREADS = 256         # segreduce.cuh:17  kSegThreads; light grid min(ceil(n/GPB), 64*SM) :160-161
+HOT_THRESHOLD = 64        # segreduce.cuh:26  kHotThreshold
+HOT_CHUNK = 2048          # segreduce.cuh:27  kHotChunk
+ROW_THREADS = 256         # gather_scatter.cuh:18 kGatherThreads; grids min(ceil(n/GPB), 64*SM)
+#                           gather_scatter.cuh:132-134 (pool), :328-330 and :349-351 (row updates)
+FWD_THREADS = 128         # embed_fm.cuh:56-57 FwdGeom; grid min(tiles, SM*ctas_per_sm) :596
+FWD_CTAS_PER_SM = 8       # embed_fm.cuh:39 K1Config default ctas_per_sm
+BWD_THREADS = 256         # embed_fm.cuh:634 kBwdThreads (dense-part samples per CTA = 256/TPR :675)
+BWD_DENSE_CTAS_PER_SM = 2  # embed_fm.cuh:792 bwd_dense_grid() = 2*SM
+DENSE_CHUNK = 8           # embed_fm.cuh:666 kDenseChunk
+BWD_WARPS = 8             # embed_fm.cuh:676 kWarps = kBwdThreads/32
+RED_LANES = 32            # embed_fm.cuh:758 kRedLanes; 4-in-flight loop while g + 3*32 < G :768
+DOT_WARPS = 4             # dot_interact.cuh:24 kDotWarps; shrink while > 96 KB b200rec.cu:607-608
+DOT_CTAS_PER_SM = 8       # b200rec.cu:612
+CROSS_ROW_SLICES = 264    # cross.cuh:42 kCrossRowSlices
+TOWER_ROW_SLICES = 528    # tower.cuh:337 kTowerRowSlices; TX/TY tower.cuh:382-384
+TOWER_THREADS = 256       # tower.cuh:21
+TOWER_UNROLL = 4          # tower.cuh:103 kBwdUnroll
+STREAM_CTAS_PER_SM = 16   # b200rec.cu:577,589,642 (cvm, hash_keys: 256-thread CTAs)
+
+
+def _ops():
+    from paddlerec_b200 import ops
+    return ops
+
+
+def _sm():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def _cdiv(a, b):
+    return -(-a // b)
+
+
+def row_shape(D):
+    """pick_row_shape, common.cuh:223-232: (VEC floats per lane, TPR lanes per row)."""
+    vec = 4 if D % 4 == 0 else (2 if D % 2 == 0 else 1)
+    chunks = D // vec
+    tpr = 1
+    while tpr < chunks:
+        tpr <<= 1
+    return vec, tpr
+
+
+def assert_loops(what, iters):
+    """Every CTA / warp / lane group of `what` makes at least MIN_ITERS passes."""
+    print("[iterations] %s: %d" % (what, iters))
+    assert iters >= MIN_ITERS, "%s: only %d passes per CTA; the size no longer makes the grid loop" % (
+        what, iters)
+
+
+def assert_within(got, want, bound, what):
+    """Element-wise |got - want| <= bound (all float64 on the device)."""
+    got = got.double()
+    assert got.shape == want.shape, (what, got.shape, want.shape)
+    err = (got - want).abs()
+    bad = ~(err <= bound)
+    if bool(bad.any()):
+        i = int(torch.argmax((err - bound).reshape(-1)))
+        raise AssertionError("%s: %d / %d entries out of bound; worst at flat index %d: got %.9g want "
+                             "%.9g bound %.3g" % (what, int(bad.sum()), bad.numel(), i,
+                                                  float(got.reshape(-1)[i]), float(want.reshape(-1)[i]),
+                                                  float(bound.reshape(-1)[i])))
+
+
+@pytest.fixture(autouse=True)
+def hbm_budget(request):
+    """Each test allocates at most ~12 GB; skip when the shared GPU has less free."""
+    torch.cuda.synchronize()
+    torch.cuda.empty_cache()
+    free, _ = torch.cuda.mem_get_info()
+    if free < 14e9:
+        pytest.skip("needs ~14 GB of free HBM (%.1f GB free)" % (free / 1e9))
+    torch.cuda.reset_peak_memory_stats()
+    yield
+    torch.cuda.synchronize()
+    peak = torch.cuda.max_memory_allocated()
+    print("[peak] %s: %.2f GB" % (request.node.name, peak / 1e9))
+    assert peak <= 12.5e9, "%s allocated %.1f GB" % (request.node.name, peak / 1e9)
+
+
+def seg_chain(counts, D):
+    """Longest fp32 chain of one merged row in launch_seg_reduce (segreduce.cuh): a segment of
+    <= 64 positions is summed sequentially by one lane group (k = count); a hot one is cut into
+    2048-position chunks, each summed by GPB groups striding the chunk (ceil(2048/GPB) adds), a
+    log2(GPB)-level shared-memory tree, and seg_combine_kernel adds the chunk partials in order
+    (one add per chunk)."""
+    _, tpr = row_shape(D)
+    gpb = SEG_THREADS // tpr
+    hot = counts > HOT_THRESHOLD
+    k_hot = _cdiv(HOT_CHUNK, gpb) + int(math.log2(gpb)) + (counts + HOT_CHUNK - 1) // HOT_CHUNK
+    return torch.where(hot, k_hot, counts).double()
+
+
+# ================================================================================================
+# 1. DIN attention (din_attn.cuh): forward scores kernel and fused backward, persistent over tiles
+# ================================================================================================
+def _din_params(E, g):
+    W1 = torch.randn(4 * E, DIN_H1, generator=g, device=DEV) / (4 * E) ** 0.5
+    b1 = torch.randn(DIN_H1, generator=g, device=DEV) * 0.1
+    W2 = torch.randn(DIN_H1, DIN_H2, generator=g, device=DEV) / DIN_H1 ** 0.5
+    b2 = torch.randn(DIN_H2, generator=g, device=DEV) * 0.1
+    W3 = torch.randn(DIN_H2, 1, generator=g, device=DEV) / DIN_H2 ** 0.5
+    b3 = torch.randn(1, generator=g, device=DEV) * 0.1
+    return [W1, b1, W2, b2, W3, b3]
+
+
+def _din_reference(hist, tseq, mask, params, dout, L_tiles_k):
+    """fp64 on the device, chunked over samples.  Returns, per output and gradient:
+      want  nets.din_attention_unit and its autograd gradients;
+      bound k * 2^-24 * M + Ep, where M is the output recomputed with every factor replaced by its
+            absolute value (the sum|terms| of its own summation, chain length k from L_tiles_k) and
+            Ep is the first-order propagation, position by position, of the fp32 errors of the
+            factors the kernels recompute (z1, z2, the softmax weights w, <dout, h>, da, dz2, g).
+    Forward error model (u = 2^-24; sigmoid by __expf, add and divide: 4u absolute on z <= 1):
+      a1 = h Wac + (h*t) Wd + tb      e_a1 = (3E + 4) u M_a1   (tb: E-term addmm; 2E fmas)
+      z1 = sigmoid(a1)                e_z1 = e_a1 / 4 + 4u     (sigmoid' <= 1/4)
+      a2 = z1 W2 + b2                 e_a2 = 82 u M_a2 + e_z1 |W2|
+      z2, s = scale (z2 W3 + b3)      e_s  = scale (44 u M_s + e_z2 |W3|)
+      w = softmax(s)                  |dw_l| <= w_l (2 max_l e_s + (ceil(L/128) + 12) u)"""
+    B, L, E = hist.shape
+    scale = E ** -0.5
+    P64 = [p.double().requires_grad_(True) for p in params]
+    W1, b1, W2, b2, W3, b3 = [p.detach() for p in P64]
+    Wa, Wb, Wc, Wd = W1[:E], W1[E:2 * E], W1[2 * E:3 * E], W1[3 * E:]
+    aWac, aWd, aWbc, aW2, aW3 = (Wa + Wc).abs(), Wd.abs(), (Wb - Wc).abs(), W2.abs(), W3.abs().reshape(-1)
+    f64 = dict(dtype=torch.float64, device=DEV)
+    want = {"out": torch.empty(B, E, **f64), "dhist": torch.empty(B, L, E, **f64),
+            "dtseq": torch.empty(B, E, **f64)}
+    bound = {k: torch.empty_like(v) for k, v in want.items()}
+    pgrad = [torch.zeros_like(p) for p in P64]
+    acc = {k: torch.zeros(E, DIN_H1, **f64) for k in ("MWa", "EWa", "MWb", "EWb", "MWd", "EWd")}
+    acc.update({k: torch.zeros(DIN_H1, **f64) for k in ("Mb1", "Eb1")})
+    acc.update({k: torch.zeros(DIN_H1, DIN_H2, **f64) for k in ("MW2", "EW2")})
+    acc.update({k: torch.zeros(DIN_H2, **f64) for k in ("Mb2", "Eb2", "MW3", "EW3")})
+    acc.update({k: torch.zeros((), **f64) for k in ("Mb3", "Eb3")})
+    wsum = torch.empty(B, **f64)
+    k_out, k_dhist, k_dtseq, k_cta, k_B, k_P = L_tiles_k
+    chunk = max(1, (1 << 24) // (L * 4 * E))
+    for s in range(0, B, chunk):
+        e = min(B, s + chunk)
+        h = hist[s:e].double().requires_grad_(True)
+        t = tseq[s:e].double().requires_grad_(True)
+        m = mask[s:e] if mask is not None else None
+        go = dout[s:e].double()
+        o = nets.din_attention_unit(h, t, m, *P64)
+        gs = torch.autograd.grad(o, [h, t] + P64, go)
+        want["out"][s:e] = o.detach()
+        want["dhist"][s:e] = gs[0]
+        want["dtseq"][s:e] = gs[1]
+        for a, gg in zip(pgrad, gs[2:]):
+            a += gg
+        with torch.no_grad():
+            h, t = h.detach(), t.detach()
+            tt = t.unsqueeze(1).expand_as(h)
+            ah, at, aht = h.abs(), t.abs(), (h * tt).abs()
+            c = torch.cat([h, tt, h - tt, h * tt], 2)
+            z1 = torch.sigmoid(c @ W1 + b1)
+            z2 = torch.sigmoid(z1 @ W2 + b2)
+            sc = (z2 @ W3 + b3).squeeze(2)
+            if m is not None:
+                sc = sc + m.reshape(sc.shape).double()
+            w = torch.softmax(sc * scale, 1)
+            wsum[s:e] = w.sum(1)
+            live = w > 0
+            # forward errors
+            Ma1 = ah @ aWac + aht @ aWd + (at @ aWbc + b1.abs()).unsqueeze(1)
+            ez1 = (3 * E + 4) * U * Ma1 / 4 + 4 * U
+            ez2 = (82 * U * (z1 @ aW2 + b2.abs()) + ez1 @ aW2) / 4 + 4 * U
+            es = scale * (44 * U * (z2 @ aW3 + b3.abs()) + ez2 @ aW3) * live
+            dlw = 2 * es.max(1, keepdim=True).values + (_cdiv(L, 128) + 12) * U
+            Ew = w * dlw
+            # backward values, magnitudes M and propagated errors Ep
+            dw = (h * go.unsqueeze(1)).sum(2)
+            Mdw = (ah * go.abs().unsqueeze(1)).sum(2)
+            Edw = (E + 6) * U * Mdw
+            dot = (w * dw).sum(1, keepdim=True)
+            Edot = (Ew * dw.abs() + w * Edw).sum(1, keepdim=True) + (_cdiv(L, 128) + 8) * U * (w * dw.abs()).sum(1, keepdim=True)
+            da = scale * w * (dw - dot)
+            Mda = scale * w * (Mdw + (w * Mdw).sum(1, keepdim=True))
+            Eda = scale * (Ew * (dw.abs() + dot.abs()) + w * (Edw + Edot)) + 3 * U * Mda
+            d2 = z2 * (1 - z2)
+            Mdz2 = Mda.unsqueeze(2) * aW3 * d2
+            dz2 = da.unsqueeze(2) * W3.reshape(-1) * d2
+            Edz2 = (Eda.unsqueeze(2) * d2 + da.abs().unsqueeze(2) * ez2) * aW3 + 4 * U * Mdz2
+            d1 = z1 * (1 - z1)
+            q = dz2 @ W2.t()
+            Mq = Mdz2 @ aW2.t()
+            Mg = Mq * d1
+            Eg = (Edz2 @ aW2.t() + 41 * U * Mq) * d1 + q.abs() * ez1 + 2 * U * Mg
+            # outputs
+            bound["out"][s:e] = k_out * U * (w.unsqueeze(2) * ah).sum(1) + (Ew.unsqueeze(2) * ah).sum(1)
+            MgWd, EgWd = Mg @ aWd.t(), Eg @ aWd.t()
+            bound["dhist"][s:e] = (k_dhist * U * (w.unsqueeze(2) * go.abs().unsqueeze(1) + Mg @ aWac.t()
+                                                  + MgWd * tt.abs())
+                                   + Ew.unsqueeze(2) * go.abs().unsqueeze(1) + Eg @ aWac.t() + EgWd * tt.abs())
+            bound["dtseq"][s:e] = (k_dtseq * U * ((MgWd * ah).sum(1) + Mg.sum(1) @ aWbc.t())
+                                   + (EgWd * ah).sum(1) + Eg.sum(1) @ aWbc.t())
+            flat = lambda x: x.reshape(-1, x.shape[-1])  # noqa: E731
+            acc["MWa"] += flat(ah).t() @ flat(Mg)
+            acc["EWa"] += flat(ah).t() @ flat(Eg)
+            acc["MWb"] += at.t() @ Mg.sum(1)
+            acc["EWb"] += at.t() @ Eg.sum(1)
+            acc["MWd"] += flat(aht).t() @ flat(Mg)
+            acc["EWd"] += flat(aht).t() @ flat(Eg)
+            acc["Mb1"] += Mg.sum((0, 1))
+            acc["Eb1"] += Eg.sum((0, 1))
+            acc["MW2"] += flat(z1).t() @ flat(Mdz2)
+            acc["EW2"] += flat(z1).t() @ flat(Edz2) + flat(ez1).t() @ flat(dz2.abs())
+            acc["Mb2"] += Mdz2.sum((0, 1))
+            acc["Eb2"] += Edz2.sum((0, 1))
+            acc["MW3"] += (z2 * Mda.unsqueeze(2)).sum((0, 1))
+            acc["EW3"] += (z2 * Eda.unsqueeze(2) + ez2 * da.abs().unsqueeze(2)).sum((0, 1))
+            acc["Mb3"] += Mda.sum()
+            acc["Eb3"] += Eda.sum()
+    a = acc
+    bWa = k_cta * U * a["MWa"] + a["EWa"]
+    bWb = k_B * U * a["MWb"] + a["EWb"]
+    bound["dW1"] = torch.cat([bWa, bWb, bWa + bWb + U * (a["MWa"] + a["MWb"]), k_cta * U * a["MWd"] + a["EWd"]], 0)
+    bound["db1"] = k_B * U * a["Mb1"] + a["Eb1"]
+    bound["dW2"] = k_cta * U * a["MW2"] + a["EW2"]
+    bound["db2"] = k_cta * U * a["Mb2"] + a["Eb2"]
+    bound["dW3"] = (k_cta * U * a["MW3"] + a["EW3"]).reshape(-1, 1)
+    bound["db3"] = (k_P * U * a["Mb3"] + a["Eb3"]).reshape(1)
+    for k, gg in zip(("dW1", "db1", "dW2", "db2", "dW3", "db3"), pgrad):
+        want[k] = gg
+    return want, bound, wsum
+
+
+def _din_case(B, L, E, seed):
+    """Runs the fused forward + backward (ops.din_attention) on B samples of L positions with a
+    mask of variable lengths, and checks every output and gradient element-wise against
+    nets.din_attention_unit in fp64 (bounds: _din_reference).
+
+    Loop: P = B*L positions in 64-position tiles, grid = min(tiles, SM) persistent CTAs
+    (din_attn.cuh:627-630, 693-694); each CTA runs `tpc` tiles and the backward keeps
+    aWac/aWd/aW2/ab2/aW3 in registers across all of them (din_attn.cuh:331-343).
+
+    Summation chains k (on top of the propagated factor errors):
+      out          L-term fma chain over the history (din_softmax_pool_kernel) + 1
+      dhist        80-term GEMMs (g Wac^T, g Wd^T) + 3 fmas
+      dtseq        L positions (atomics, any order) + 80 (g Wd^T) + 80 (addmm with dtb) + 2
+      dWa, dWd, dW2, db2, dW3   64 positions per tile x tpc tiles in a CTA's registers, then the
+                   grid partials in order (din_reduce_partials_kernel) + 16 (shuffles, products)
+      dWb, db1     B samples (torch matmul / sum over dtb) + L (dtb atomics) + 2
+      db3          B*L (torch sum of da) + 2
+    The softmax weights must sum to 1 within (ceil(L/128) + 10) roundings (128-thread sum, 5-level
+    shuffle, 4 warp partials, one division, one multiply per weight), and masked positions get
+    exactly 0."""
+    ops = _ops()
+    SM = _sm()
+    P = B * L
+    tiles = _cdiv(P, DIN_TILE)
+    grid = min(tiles, SM)
+    tpc = _cdiv(tiles, grid)
+    assert_loops("din scores fwd/bwd B=%d L=%d E=%d: tiles per CTA" % (B, L, E), tiles // grid)
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    hist = torch.randn(B, L, E, generator=g, device=DEV) * 0.5
+    tseq = torch.randn(B, E, generator=g, device=DEV) * 0.5
+    lens = torch.randint(1, L + 1, (B,), generator=g, device=DEV)
+    lens[0] = L
+    lens[1 % B] = 1
+    mask = torch.where(torch.arange(L, device=DEV).unsqueeze(0) < lens.unsqueeze(1), 0,
+                       int(-1e9)).to(torch.int64).unsqueeze(2)
+    params = _din_params(E, g)
+    dout = torch.randn(B, E, generator=g, device=DEV)
+
+    dev_in = [t.clone().requires_grad_(True) for t in [hist, tseq] + params]
+    out = ops.din_attention(dev_in[0], dev_in[1], mask, *dev_in[2:])
+    out.backward(dout)
+    _, w = ops.raw_din_attn_fwd(hist, tseq, mask, *params)
+    torch.cuda.synchronize()
+
+    ks = (L + 1, DIN_H1 + 3, L + 2 * DIN_H1 + 2, DIN_TILE * tpc + grid + 16, B + L + 2, P + 2)
+    want, bound, wsum_ref = _din_reference(hist, tseq, mask, params, dout, ks)
+    got = {"out": out, "dhist": dev_in[0].grad, "dtseq": dev_in[1].grad}
+    got.update(zip(("dW1", "db1", "dW2", "db2", "dW3", "db3"), [p.grad for p in dev_in[2:]]))
+    for name in ("out", "dhist", "dtseq", "dW1", "db1", "dW2", "db2", "dW3", "db3"):
+        assert_within(got[name], want[name], bound[name] + 1e-30, "DIN %s B=%d L=%d E=%d" % (name, B, L, E))
+    # softmax weights: normalised, masked positions exactly zero
+    assert_within(w.double().sum(1), torch.ones_like(wsum_ref),
+                  torch.full_like(wsum_ref, (_cdiv(L, 128) + 10) * U), "DIN sum of weights")
+    masked = mask.squeeze(2) != 0
+    assert bool((w[masked] == 0).all()), "masked history positions must get weight exactly 0"
+    # the fixed-order weight gradients are bit-reproducible (dtseq / dtb use atomics: excluded)
+    r1 = ops.raw_din_attn_bwd(hist, tseq, *params[:5], w, dout)
+    r2 = ops.raw_din_attn_bwd(hist, tseq, *params[:5], w, dout)
+    kernel_rows = torch.cat([torch.arange(E), torch.arange(3 * E, 4 * E)]).to(DEV)  # Wa, Wd of dW1
+    assert torch.equal(r1[2][kernel_rows], r2[2][kernel_rows]), "DIN dWac/dWd differ between runs"
+    for i in (4, 5, 6):          # dW2, db2, dW3
+        assert torch.equal(r1[i], r2[i]), "DIN fixed-order weight gradient %d differs between runs" % i
+    assert torch.equal(r1[0], r2[0]), "dhist is per position (no atomics): must be reproducible"
+
+
+def test_din_bench_shape():
+    """The DIN benchmark shape: B=4096, L=100, E=128, ~48 tiles per CTA."""
+    _din_case(4096, 100, 128, seed=1)
+
+
+@pytest.mark.parametrize("E", [4, 20, 36, 100])
+def test_din_partial_register_tiles(E):
+    """E not a multiple of 16: the last of the kreps = ceil(E/16) k-rows of the aWac/aWd register
+    tiles is partial (din_attn.cuh:344, 522-525, 604-606).  L=61 makes tiles straddle samples."""
+    L = 61
+    B = _cdiv((3 * _sm() + _sm() // 2) * DIN_TILE, L)
+    _din_case(B, L, E, seed=E)
+
+
+def test_din_longest_history():
+    """L = 8192 (the maximum: a 32 KB softmax row in shared memory) with enough samples that the
+    grid loops."""
+    L = 8192
+    B = _cdiv((3 * _sm() + _sm() // 2) * DIN_TILE, L)
+    _din_case(B, L, 32, seed=8192)
+
+
+# ================================================================================================
+# 2. Segment reduce (segreduce.cuh): hot path with several 2048-position chunks + combine
+# ================================================================================================
+HOT_LENS = [64, 65, 2048, 2049, 6145, 150001]
+
+
+def _hot_stream(n_uniform, V, g):
+    """Ids with segments of exactly HOT_LENS positions (ids 11..16), uniform traffic, and 5000
+    padding ids (0) shuffled in between, so padding sits inside the hot runs."""
+    parts = [torch.full((n,), 11 + i, dtype=torch.int64, device=DEV) for i, n in enumerate(HOT_LENS)]
+    parts.append(torch.randint(100, V, (n_uniform,), generator=g, device=DEV))
+    parts.append(torch.zeros(5000, dtype=torch.int64, device=DEV))
+    ids = torch.cat(parts)
+    return ids[torch.randperm(ids.numel(), generator=g, device=DEV)]
+
+
+def _check_segment_rows(ops, gr, rows_fn, contrib, valid_ids, D, what):
+    """rows_fn() -> merged rows; contrib [n_valid, D] fp64 per-position terms in position order;
+    checks against index_add in fp64 with the seg_chain bound, then bit-reproducibility."""
+    uniq, inv, counts = torch.unique(valid_ids, return_inverse=True, return_counts=True)
+    Uq = uniq.numel()
+    assert int(gr.num[0]) == Uq
+    assert torch.equal(gr.unique_ids[:Uq], uniq)
+    want = torch.zeros(Uq, D, dtype=torch.float64, device=DEV).index_add_(0, inv, contrib)
+    mag = torch.zeros(Uq, D, dtype=torch.float64, device=DEV).index_add_(0, inv, contrib.abs())
+    k = seg_chain(counts, D).unsqueeze(1)
+    rows = rows_fn()
+    assert_within(rows[:Uq], want, k * U * mag + 1e-30, what)
+    assert torch.equal(rows[:Uq], rows_fn()[:Uq]), what + ": not bit-reproducible"
+    return counts
+
+
+@pytest.mark.parametrize("D", [1, 2, 3, 9, 16, 40, 128])
+def test_segment_reduce_hot_chunks(D):
+    """raw_segment_reduce on segments of 64 (light), 65, 2048, 2049 (hot, 1-2 chunks), 6145
+    (4 chunks) and 150001 (74 chunks) positions plus uniform traffic and padding; every VEC/TPR
+    family.  Bound: seg_chain (light: count adds; hot: ceil(2048/GPB) + log2(GPB) + chunks)."""
+    ops = _ops()
+    chunks = [_cdiv(n, HOT_CHUNK) for n in HOT_LENS if n > HOT_THRESHOLD]
+    assert_loops("seg_combine_kernel: chunks added for the 6145-position id", chunks[-2])
+    assert_loops("seg_combine_kernel: chunks added for the 150001-position id", chunks[-1])
+    g = torch.Generator(device=DEV).manual_seed(D)
+    V = 1_000_000
+    ids = _hot_stream(100_000, V, g)
+    n = ids.numel()
+    dOut = torch.randn(n, D, generator=g, device=DEV)
+    gr = ops.raw_group_ids(ids, V, 0)
+    valid = ids != 0
+    counts = _check_segment_rows(
+        ops, gr, lambda: ops.raw_segment_reduce(dOut, gr.seg_offsets, gr.sorted_pos, gr.num, n),
+        dOut[valid].double(), ids[valid], D, "segment_reduce D=%d" % D)
+    assert sorted(counts[counts > 1000].tolist()) == [2048, 2049, 6145, 150001]
+
+
+def test_segment_reduce_light_kernel_loops():
+    """D=16 with U >= 3 * 64*SM CTAs * 64 groups distinct ids: every lane group of
+    seg_light_kernel walks >= 3 segments (segreduce.cuh:47-48, 160-161); hot ids ride along."""
+    ops = _ops()
+    D = 16
+    _, tpr = row_shape(D)
+    gpb = SEG_THREADS // tpr
+    cap = 64 * _sm() * gpb
+    Uq = 3 * cap + 1001
+    g = torch.Generator(device=DEV).manual_seed(16)
+    V = 4 * Uq
+    ids = torch.cat([torch.randperm(V - 100, generator=g, device=DEV)[:Uq] + 100,
+                     _hot_stream(0, V, g)])
+    ids = ids[torch.randperm(ids.numel(), generator=g, device=DEV)]
+    n = ids.numel()
+    grid = min(_cdiv(n, gpb), 64 * _sm())
+    assert_loops("seg_light_kernel: segments per lane group", Uq // (grid * gpb))
+    dOut = torch.randn(n, D, generator=g, device=DEV)
+    gr = ops.raw_group_ids(ids, V, 0)
+    valid = ids != 0
+    _check_segment_rows(
+        ops, gr, lambda: ops.raw_segment_reduce(dOut, gr.seg_offsets, gr.sorted_pos, gr.num, n),
+        dOut[valid].double(), ids[valid], D, "segment_reduce light loop")
+
+
+# ================================================================================================
+# 3. embed_fm backward at B=65536 with Zipf ids (hot ids of tens of thousands of positions)
+# ================================================================================================
+@pytest.mark.parametrize("D", [9, 16, 40])
+@pytest.mark.parametrize("Dn", [0, 8, 13, 17])
+def test_embed_fm_bwd_zipf(D, Dn):
+    """raw_embed_fm_bwd, two-table and fused_cols layouts, B=65536 x F=26, Zipf ids over V=1e6.
+
+    Sparse rows: per position the kernel forms fmaf(gy2, S - feat, dfeat) (2 roundings of
+    |gy2|(|S| + |feat|) + |dfeat|) and merges them in seg_chain order: k = seg_chain + 2.  dW1 is
+    the same merge of gy1 (k = seg_chain).
+    Dense part (embed_fm_bwd_dense_kernel): each lane accumulates iters = ceil(B / (2*SM*SPB))
+    samples, then log2(32/TPR) shuffles, 8 warp partials in order, and reduce_partials_kernel adds
+    ceil(G/32) partials per lane and 32 lanes: k = iters + 5 + 8 + ceil(G/32) + 32 + 3 for
+    fmaf(x, fmaf(g2, S - fe, dd), acc) terms of magnitude |x|(|g2|(|S| + |fe|) + |dd|)."""
+    ops = _ops()
+    SM = _sm()
+    B, F, V = 65536, 26, 1_000_000
+    vec, tpr = row_shape(D)
+    spb = BWD_THREADS // tpr
+    G = BWD_DENSE_CTAS_PER_SM * SM
+    assert_loops("embed_fm_bwd_dense_kernel D=%d: samples per lane" % D, B // (G * spb))
+    red_iters = len(range(0, G - 3 * RED_LANES, 4 * RED_LANES))
+    assert red_iters >= 1, "reduce_partials_kernel's 4-loads-in-flight branch is no longer reached"
+    g = torch.Generator(device=DEV).manual_seed(1000 * D + Dn)
+    r = torch.rand(B, F, generator=g, device=DEV, dtype=torch.float64)
+    ids = (V ** r).to(torch.int64).clamp_(1, V - 1)
+    ids[torch.rand(B, F, generator=g, device=DEV) < 0.02] = 0
+    N = F + Dn
+    feat = torch.randn(B, N, D, generator=g, device=DEV) * 0.1
+    S = torch.randn(B, D, generator=g, device=DEV)
+    dfeat = torch.randn(B, N, D, generator=g, device=DEV) * 0.01
+    gy1 = torch.randn(B, generator=g, device=DEV)
+    gy2 = torch.randn(B, generator=g, device=DEV)
+    dense = torch.rand(B, Dn, generator=g, device=DEV)
+    dense[torch.rand(B, Dn, generator=g, device=DEV) < 0.3] = 0
+    gr = ops.raw_group_ids(ids, V, 0)
+    args = (feat, S, dfeat, gy1, gy2, dense, gr.seg_offsets, gr.sorted_pos, gr.num, F)
+
+    flat = ids.reshape(-1)
+    valid = flat != 0
+    b_of = torch.arange(B, device=DEV).repeat_interleave(F)[valid]
+    fe = feat[:, :F].reshape(-1, D)[valid].double()
+    dd = dfeat[:, :F].reshape(-1, D)[valid].double()
+    g2 = gy2.double()[b_of].unsqueeze(1)
+    Sb = S.double()[b_of]
+    uniq, inv, counts = torch.unique(flat[valid], return_inverse=True, return_counts=True)
+    Uq = uniq.numel()
+    hot_chunks = _cdiv(int(counts.max()), HOT_CHUNK)
+    assert_loops("embed_fm_bwd seg_combine_kernel: chunks of the hottest id", hot_chunks)
+    z = lambda *s: torch.zeros(*s, dtype=torch.float64, device=DEV)  # noqa: E731
+    want = z(Uq, D).index_add_(0, inv, g2 * (Sb - fe) + dd)
+    mag = z(Uq, D).index_add_(0, inv, g2.abs() * (Sb.abs() + fe.abs()) + dd.abs())
+    del fe, dd, Sb
+    want1 = z(Uq).index_add_(0, inv, gy1.double()[b_of])
+    mag1 = z(Uq).index_add_(0, inv, gy1.double().abs()[b_of])
+    k = seg_chain(counts, D)
+
+    dW, dW1, ddw, ddw1 = ops.raw_embed_fm_bwd(*args)
+    assert_within(dW[:Uq], want, (k + 2).unsqueeze(1) * U * mag + 1e-30, "dW rows D=%d Dn=%d" % (D, Dn))
+    assert_within(dW1[:Uq], want1, k * U * mag1 + 1e-30, "dW1 rows D=%d Dn=%d" % (D, Dn))
+    if Dn > 0:
+        x = dense.double().unsqueeze(2)
+        fd, dfd = feat[:, F:].double(), dfeat[:, F:].double()
+        g2b = gy2.double().reshape(B, 1, 1)
+        Sd = S.double().unsqueeze(1)
+        wdw = (x * (g2b * (Sd - fd) + dfd)).sum(0)
+        mdw = (x * (g2b.abs() * (Sd.abs() + fd.abs()) + dfd.abs())).sum(0)
+        kd = _cdiv(B, G * spb) + int(math.log2(32 // tpr)) + BWD_WARPS + _cdiv(G, RED_LANES) + RED_LANES
+        assert_within(ddw, wdw, (kd + 3) * U * mdw + 1e-30, "ddense_w D=%d Dn=%d" % (D, Dn))
+        wd1 = (dense.double() * gy1.double().unsqueeze(1)).sum(0)
+        md1 = (dense.double() * gy1.double().abs().unsqueeze(1)).sum(0)
+        kd1 = _cdiv(B, G * spb) + 5 + BWD_WARPS + _cdiv(G, RED_LANES) + RED_LANES + 1
+        assert_within(ddw1, wd1, kd1 * U * md1 + 1e-30, "ddense_w1 D=%d Dn=%d" % (D, Dn))
+    # deterministic, and the fused layout [D | g1 | zeros] holds exactly the same numbers
+    dW_b, dW1_b, ddw_b, ddw1_b = ops.raw_embed_fm_bwd(*args)
+    assert torch.equal(dW[:Uq], dW_b[:Uq]) and torch.equal(dW1[:Uq], dW1_b[:Uq])
+    assert torch.equal(ddw, ddw_b) and torch.equal(ddw1, ddw1_b)
+    Gc = ops.fused_grad_cols(D)
+    dWf, none, ddw_f, _ = ops.raw_embed_fm_bwd(*args, fused_cols=Gc)
+    assert none is None
+    assert torch.equal(dWf[:Uq, :D], dW[:Uq]) and torch.equal(dWf[:Uq, D], dW1[:Uq])
+    assert not dWf[:Uq, D + 1:].any(), "zero_pad columns of the fused rows must be written as 0"
+    assert torch.equal(ddw_f, ddw)
+
+
+# ================================================================================================
+# 4. DLRM dot interaction (dot_interact.cuh): one warp per sample, persistent grid
+# ================================================================================================
+def _dot_warps(N, d, bwd):
+    """dot_interact_launch, b200rec.cu:605-608 (v1 path)."""
+    pitch = d + 1
+    per_warp = 4 * (N * pitch + (N * N if bwd else 0))
+    warps = DOT_WARPS
+    while warps > 1 and warps * per_warp > 96 * 1024:
+        warps >>= 1
+    return warps
+
+
+def _dot_ref(T, dR, self_interaction, chunk=4096):
+    """nets.dot_interact in fp64 (value and autograd gradient) and the same on |T| with |dR| as
+    the magnitude, chunked over samples."""
+    outs = [[], [], [], []]
+    for s in range(0, T.shape[0], chunk):
+        for j, src in enumerate((T[s:s + chunk], T[s:s + chunk].abs())):
+            Tl = src.double().requires_grad_(True)
+            R = nets.dot_interact(Tl, self_interaction)
+            gT, = torch.autograd.grad(R, Tl, (dR[s:s + chunk] if j == 0 else dR[s:s + chunk].abs()).double())
+            outs[j].append(R.detach())
+            outs[2 + j].append(gT)
+    return [torch.cat(o) for o in outs]
+
+
+@pytest.mark.parametrize("B,N,d", [(65536, 27, 16), (16384, 128, 4), (8192, 27, 256)])
+@pytest.mark.parametrize("self_interaction", [False, True])
+def test_dot_interact_fwd_bwd(B, N, d, self_interaction):
+    """Forward: each pair is a d-term fma chain (k = d) of magnitude sum|T_i||T_j|.  Backward:
+    dT[i,c] = sum_j dZ[i,j] T[j,c] (+ dR for the x row): k = N + 1.  No atomics: bit-identical on
+    a second run."""
+    ops = _ops()
+    SM = _sm()
+    for bwd in (False, True):
+        warps = _dot_warps(N, d, bwd)
+        grid = min(_cdiv(B, warps), DOT_CTAS_PER_SM * SM)
+        assert_loops("dot_interact %s B=%d N=%d d=%d (%d warps/CTA): samples per warp"
+                     % ("bwd" if bwd else "fwd", B, N, d, warps), B // (grid * warps))
+    g = torch.Generator(device=DEV).manual_seed(B + N + d + self_interaction)
+    T = torch.randn(B, N, d, generator=g, device=DEV)
+    dR = torch.randn(B, ops.dot_interact_width(N, d, self_interaction), generator=g, device=DEV)
+    R = ops.raw_dot_interact_fwd(T, self_interaction)
+    dT = ops.raw_dot_interact_bwd(T, dR, self_interaction)
+    wR, mR, wT, mT = _dot_ref(T, dR, self_interaction)
+    assert_within(R, wR, d * U * mR + 1e-30, "dot_interact fwd")
+    assert_within(dT, wT, (N + 1) * U * mT + 1e-30, "dot_interact bwd")
+    assert torch.equal(R[:, :d], T[:, N - 1])
+    assert torch.equal(ops.raw_dot_interact_fwd(T, self_interaction), R)
+    assert torch.equal(ops.raw_dot_interact_bwd(T, dR, self_interaction), dT)
+
+
+@pytest.mark.skipif(os.environ.get("B200REC_TEST_EXPERIMENTAL") != "1",
+                    reason="experimental K6 v2 kernels: opt in with B200REC_TEST_EXPERIMENTAL=1")
+@pytest.mark.parametrize("self_interaction", [False, True])
+def test_dot_interact_v2_matches_v1_when_warps_loop(self_interaction, monkeypatch):
+    """v2's cp.async double buffer is only used when a warp loops: B=65536 makes every warp run
+    ~15 samples.  Same products in the same order: bit-identical to v1."""
+    ops = _ops()
+    B, N, d = 65536, 27, 16
+    g = torch.Generator(device=DEV).manual_seed(27 + self_interaction)
+    T = torch.randn(B, N, d, generator=g, device=DEV)
+    dR = torch.randn(B, ops.dot_interact_width(N, d, self_interaction), generator=g, device=DEV)
+    monkeypatch.delenv("B200REC_K6_V2", raising=False)
+    R1, dT1 = ops.raw_dot_interact_fwd(T, self_interaction), ops.raw_dot_interact_bwd(T, dR, self_interaction)
+    monkeypatch.setenv("B200REC_K6_V2", "1")
+    R2, dT2 = ops.raw_dot_interact_fwd(T, self_interaction), ops.raw_dot_interact_bwd(T, dR, self_interaction)
+    assert torch.equal(R1, R2) and torch.equal(dT1, dT2)
+
+
+# ================================================================================================
+# 5. CrossNet K3 (cross.cuh): row slices accumulate the bias gradient over many rows
+# ================================================================================================
+@pytest.mark.parametrize("C", [1560, 351])
+def test_cross_v2_at_scale(C):
+    """B=65536: each of the 264 row slices of cross_v2_bwd_kernel walks ~248 rows.
+    dxw = dout*x0 and dx0 = dout*(xw + bias) are single correctly-rounded fp32 operations: equal to
+    torch's fp32 result bit for bit (hence within 2^-24 relative of fp64).
+    out = fmaf(x0, xw + bias, xl): 2 roundings of |x0|(|xw| + |bias|) + |xl|.
+    dbias: each slice adds ceil(B/264) rows in order, reduce_partials_kernel adds ceil(264/32)
+    per lane then 32 lanes: k = ceil(B/264) + 9 + 32 + 1 of sum|dout x0|."""
+    ops = _ops()
+    B = 65536
+    vec = 4 if C % 4 == 0 else 1
+    assert_loops("cross_v2_bwd_kernel C=%d: rows per slice" % C, B // CROSS_ROW_SLICES)
+    total = B * (C // vec)
+    grid = min(_cdiv(total, 256), 16 * _sm())
+    assert_loops("cross_v2_fwd_kernel C=%d: elements per thread" % C, total // (grid * 256))
+    g = torch.Generator(device=DEV).manual_seed(C)
+    x0, xl, xw, dout = (torch.randn(B, C, generator=g, device=DEV) for _ in range(4))
+    bias = torch.randn(C, generator=g, device=DEV)
+    out = ops.raw_cross_v2_fwd(x0, xl, xw, bias)
+    d = lambda t: t.double()  # noqa: E731
+    assert_within(out, d(xl) + d(x0) * (d(xw) + d(bias)),
+                  2 * U * (d(x0).abs() * (d(xw).abs() + d(bias).abs()) + d(xl).abs()), "cross fwd")
+    del out
+    dxw, dx0, dbias = ops.raw_cross_v2_bwd(dout, x0, xw, bias)
+    assert torch.equal(dxw, dout * x0)
+    assert torch.equal(dx0, dout * (xw + bias))
+    k = _cdiv(B, CROSS_ROW_SLICES) + _cdiv(CROSS_ROW_SLICES, RED_LANES) + RED_LANES + 1
+    prod = d(dout) * d(x0)
+    assert_within(dbias, prod.sum(0), k * U * prod.abs().sum(0), "cross dbias C=%d" % C)
+    assert torch.equal(ops.raw_cross_v2_bwd(dout, x0, xw, bias)[2], dbias)
+
+
+# ================================================================================================
+# 6. tower_relu_bwd_split (tower.cuh): 4-row unrolled main loop + tail, db through 528 slices
+# ================================================================================================
+@pytest.mark.parametrize("N", [1, 7, 400])
+@pytest.mark.parametrize("masked", [False, True])
+def test_tower_split_bwd_at_scale(N, masked):
+    """raw_tc_split_bwd at M=65536: g = dy * (mask_hi > 0) written as bf16 planes [hi | lo] (bit
+    exact: the same two roundings torch does) and db = column sums of g.  A thread walks
+    rows = M / row_step rows (row_step = 528 * TY), >= 3 passes of the 4-row unrolled loop plus the
+    tail; reduce_partials_kernel runs its 4-in-flight loop over the 528 partials.
+    db: k = ceil(M/row_step) + TY (block rows in order) + ceil(528/32) + 32 of sum|g|."""
+    ops = _ops()
+    M = 65536
+    ld = ops.plane_ld(N)
+    v4 = N % 4 == 0 and ld % 4 == 0
+    chunks = N // 4 if v4 else N
+    tx = 32
+    while tx < chunks and tx < TOWER_THREADS:
+        tx <<= 1
+    ty = TOWER_THREADS // tx
+    row_step = min(TOWER_ROW_SLICES, M) * ty
+    assert_loops("tower_relu_bwd_split N=%d: unrolled 4-row passes per thread" % N,
+                 (M // row_step) // TOWER_UNROLL)
+    assert (M // row_step) % TOWER_UNROLL != 0, "the tail loop should run too"
+    assert_loops("reduce_partials_kernel over %d partials: 4-in-flight passes of lane 0"
+                 % TOWER_ROW_SLICES, len(range(0, TOWER_ROW_SLICES - 3 * RED_LANES, 4 * RED_LANES)))
+    g = torch.Generator(device=DEV).manual_seed(N + masked)
+    dy = torch.randn(M, N, generator=g, device=DEV)
+    mp = ops.raw_tc_split(torch.randn(M, N, generator=g, device=DEV).clamp_min(0)) if masked else None
+    gp, db = ops.raw_tc_split_bwd(dy, mp)
+    gw = torch.where(mp[:, :N].float() > 0, dy, torch.zeros_like(dy)) if masked else dy
+    hi = gw.to(torch.bfloat16)
+    lo = (gw - hi.float()).to(torch.bfloat16)
+    assert torch.equal(gp[:, :N], hi) and torch.equal(gp[:, ld:ld + N], lo)
+    k = _cdiv(M, row_step) + ty + _cdiv(TOWER_ROW_SLICES, RED_LANES) + RED_LANES
+    assert_within(db, gw.double().sum(0), k * U * gw.double().abs().sum(0), "split bwd db N=%d" % N)
+    assert torch.equal(ops.raw_tc_split_bwd(dy, mp)[1], db)
+    if masked and N == 400:       # the older entry point shares the launcher: same planes and db
+        act = ops.raw_tower_split(torch.randn(M, N, generator=g, device=DEV), None, True)
+        dz, db2 = ops.raw_tower_relu_bwd_split(dy, act)
+        gw2 = torch.where(act[:, :N].float() > 0, dy, torch.zeros_like(dy))
+        hi2 = gw2.to(torch.bfloat16)
+        assert torch.equal(dz[:, :N], hi2) and torch.equal(dz[:, N:], (gw2 - hi2.float()).to(torch.bfloat16))
+        assert_within(db2, gw2.double().sum(0), k * U * gw2.double().abs().sum(0), "tower bwd db")
+
+
+# ================================================================================================
+# 7. Row updates (gather_scatter.cuh) at U ~ 3x the grid's capacity, against oracle/optim.py
+# ================================================================================================
+@pytest.mark.parametrize("D", [9, 16])
+def test_row_updates_at_scale(D):
+    """row_update_kernel / row_adagrad_kernel: grid = min(ceil(U/GPB), 64*SM), so each lane group
+    updates >= 3 rows.  Bounds (per element, u = 2^-24):
+      sgd      fmaf(-lr, g, w) with lr rounded to fp32: 2u (|w| + |lr g|)
+      adam     m: 3 roundings + 2 fp32 parameters per step -> 10u of m's magnitude after 2 steps;
+               v: 12u (all terms positive); w: per step 1u |w| plus the update lr_t m/(sqrt v + eps)
+               with m's error and 16 roundings (sqrt, add, div, mul, sub, lr_t, eps_t, half of v's)
+      adagrad  g2sum: (D + 8)u per step (positive terms); w: per step 1u |w| + (D + 16)u |lr g s|
+      rows_to_dense  zeros + g: exact copies
+    Untouched rows (and their moments) must stay bit-identical."""
+    ops = _ops()
+    vec, tpr = row_shape(D)
+    gpb = ROW_THREADS // tpr
+    cap = 64 * _sm() * gpb
+    Uq = 3 * cap + 77
+    grid = min(_cdiv(Uq, gpb), 64 * _sm())
+    assert_loops("row updates D=%d: rows per lane group" % D, Uq // (grid * gpb))
+    V = Uq + Uq // 4
+    g = torch.Generator(device=DEV).manual_seed(D)
+    rows = torch.randperm(V, generator=g, device=DEV)[:Uq].sort().values
+    val = torch.randn(Uq, D, generator=g, device=DEV)
+    num = torch.tensor([Uq, Uq], dtype=torch.int32, device=DEV)
+    sr = ops.SelectedRows(rows, val, num, V)
+    untouched = torch.ones(V, dtype=torch.bool, device=DEV)
+    untouched[rows] = False
+    W0 = torch.randn(V, D, generator=g, device=DEV)
+    Wh = W0[rows].double().cpu().numpy()
+    gh = val.double().cpu().numpy()
+    idx = np.arange(Uq)
+    t64 = lambda a: torch.from_numpy(a).to(DEV)  # noqa: E731
+
+    dense = sr.to_dense()
+    assert torch.equal(dense[rows], val) and not dense[untouched].any()
+    del dense
+
+    W = W0.clone()
+    ops.raw_sparse_sgd(W, sr, 0.1)
+    want = t64(ooptim.sgd(Wh, idx, gh, 0.1))
+    assert_within(W[rows], want, 2 * U * (want.abs() + 0.1 * t64(gh).abs()), "sgd")
+    assert torch.equal(W[untouched], W0[untouched])
+
+    W, m, v = W0.clone(), torch.zeros_like(W0), torch.zeros_like(W0)
+    Wr, mr, vr = Wh, np.zeros_like(Wh), np.zeros_like(Wh)
+    mm = np.zeros_like(Wh)
+    upd_mag = np.zeros_like(Wh)
+    b1, b2, eps, lr = 0.9, 0.999, 1e-8, 1e-3
+    for t in (1, 2):
+        ops.raw_sparse_adam(W, m, v, sr, lr, b1, b2, eps, b1 ** t, b2 ** t)
+        Wr, mr, vr = ooptim.adam_lazy(Wr, mr, vr, idx, gh, lr, b1, b2, eps, t)
+        mm = b1 * mm + (1 - b1) * np.abs(gh)
+        lr_t = lr * np.sqrt(1 - b2 ** t) / (1 - b1 ** t)
+        upd_mag += lr_t * (10 * mm + 16 * np.abs(mr)) / (np.sqrt(vr) + eps * np.sqrt(1 - b2 ** t))
+    assert_within(m[rows], t64(mr), 10 * U * t64(mm), "adam m")
+    assert_within(v[rows], t64(vr), 12 * U * t64(vr), "adam v")
+    assert_within(W[rows], t64(Wr), U * (2 * t64(np.abs(Wr)) + t64(upd_mag)), "adam W")
+    assert torch.equal(W[untouched], W0[untouched])
+    assert not m[untouched].any() and not v[untouched].any()
+
+    W, g2 = W0.clone(), torch.zeros(V, device=DEV)
+    Wr, g2r = Wh, np.zeros(Uq)
+    upd_mag = np.zeros_like(Wh)
+    lr, g0, lo, hi = 0.05, 3.0, -2.5, 2.5
+    for _ in range(2):
+        upd_mag += (D + 16) * lr * np.abs(gh) * np.sqrt(g0 / (g0 + g2r))[:, None]
+        ops.raw_sparse_adagrad(W, g2, sr, lr, g0, lo, hi)
+        Wr, g2r = ooptim.adagrad_row(Wr, g2r, idx, gh, lr, g0, lo, hi)
+    assert_within(g2[rows], t64(g2r), 2 * (D + 8) * U * t64(g2r), "adagrad g2sum")
+    assert_within(W[rows], t64(Wr), U * (2 * t64(np.abs(Wr)) + t64(upd_mag)), "adagrad W")
+    assert torch.equal(W[untouched], W0[untouched]) and not g2[untouched].any()
+
+
+# ================================================================================================
+# 8. gather_pool_sum (gather_scatter.cuh) forward with n_bags ~ 3x capacity, and its backward
+# ================================================================================================
+@pytest.mark.parametrize("D", [9, 16])
+def test_gather_pool_sum_at_scale(D):
+    """gather_pool_kernel: one lane group per bag, grid = min(ceil(n_bags/GPB), 64*SM), so each group
+    pools >= 3 bags.  A bag of len keys is a chain of len adds: k = len of sum|W rows|.  Empty bags
+    are exactly 0; padding and out-of-range keys are skipped (and counted).  Backward: the pooled
+    gradient through raw_segment_reduce(row_of_pos=bag_of_pos) with a hot key of many chunks,
+    seg_chain bound, bit-reproducible."""
+    ops = _ops()
+    vec, tpr = row_shape(D)
+    gpb = ROW_THREADS // tpr
+    cap = 64 * _sm() * gpb
+    n_bags = 3 * cap + 123
+    grid = min(_cdiv(n_bags, gpb), 64 * _sm())
+    assert_loops("gather_pool_kernel D=%d: bags per lane group" % D, n_bags // (grid * gpb))
+    V = 100_000
+    g = torch.Generator(device=DEV).manual_seed(D)
+    lens = torch.randint(0, 6, (n_bags,), generator=g, device=DEV)
+    lens[::97] = 0
+    offsets = torch.zeros(n_bags + 1, dtype=torch.int64, device=DEV)
+    offsets[1:] = torch.cumsum(lens, 0)
+    nnz = int(offsets[-1])
+    keys = torch.randint(0, V, (nnz,), generator=g, device=DEV)
+    keys[::25] = 17
+    keys[5::1001] = V + 3
+    W = torch.randn(V, D, generator=g, device=DEV)
+    ops.raw_oob_count()
+    out, bag_of_pos = ops.raw_gather_pool_sum(W, keys, offsets, 0)
+    assert ops.raw_oob_count() == int((keys >= V).sum())
+    bag = torch.arange(n_bags, device=DEV).repeat_interleave(lens)
+    assert torch.equal(bag_of_pos[:nnz], bag.to(torch.int32))
+    ok = (keys != 0) & (keys < V)
+    Wd = W.double()
+    want = torch.zeros(n_bags, D, dtype=torch.float64, device=DEV).index_add_(0, bag[ok], Wd[keys[ok]])
+    mag = torch.zeros_like(want).index_add_(0, bag[ok], Wd[keys[ok]].abs())
+    assert_within(out, want, lens.double().unsqueeze(1) * U * mag + 1e-30, "gather_pool_sum D=%d" % D)
+    assert not out[lens == 0].any()
+    # backward
+    dout = torch.randn(n_bags, D, generator=g, device=DEV)
+    gr = ops.raw_group_ids(keys, V, 0)
+    counts = _check_segment_rows(
+        ops, gr, lambda: ops.raw_segment_reduce(dout, gr.seg_offsets, gr.sorted_pos, gr.num, nnz,
+                                                row_of_pos=bag_of_pos),
+        dout.double()[bag[ok]], keys[ok], D, "gather_pool_sum backward D=%d" % D)
+    assert_loops("pooled backward: chunks of the hot key", _cdiv(int(counts.max()), HOT_CHUNK))
+
+
+# ================================================================================================
+# 9. embed_fm forward (embed_fm.cuh): persistent tiles with the double-buffered id prefetch
+# ================================================================================================
+@pytest.mark.parametrize("D", [9, 16, 40])
+@pytest.mark.parametrize("fused", [False, True])
+def test_embed_fm_fwd_at_scale(D, fused):
+    """B >= 65536 (more for D=16, so that every CTA runs >= 3 tiles: grid = min(tiles, 8*SM),
+    tile = 128/TPR samples), V=1e6.  The WHOLE feat is compared with torch.equal (gathers are
+    copies; dense rows one fp32 product).  S: N-term sums, k = N of sum|feat|; y1: N terms, one of
+    which a product, k = N + 2; y2 = 0.5 sum_d (S_d^2 - Q_d): the S error doubles through the
+    square, so k = 4N + 2D + 8 of 0.5 sum_d ((sum_f |feat|)^2 + Q_d)."""
+    ops = _ops()
+    SM = _sm()
+    F, Dn, V = 26, 13, 1_000_000
+    N = F + Dn
+    _, tpr = row_shape(D)
+    spb = FWD_THREADS // tpr
+    B = max(65536, 3 * FWD_CTAS_PER_SM * SM * spb)
+    tiles = _cdiv(B, spb)
+    grid = min(tiles, FWD_CTAS_PER_SM * SM)
+    assert_loops("embed_fm_fwd_kernel D=%d B=%d: tiles per CTA" % (D, B), tiles // grid)
+    g = torch.Generator(device=DEV).manual_seed(D + 100 * fused)
+    ids = torch.randint(1, V, (B, F), generator=g, device=DEV)
+    ids[torch.rand(B, F, generator=g, device=DEV) < 0.02] = 0
+    dense = torch.rand(B, Dn, generator=g, device=DEV)
+    W = torch.randn(V, D, generator=g, device=DEV) * 0.1
+    W1 = torch.randn(V, 1, generator=g, device=DEV) * 0.1
+    dense_w = torch.randn(Dn, D, generator=g, device=DEV) * 0.1
+    dense_w1 = torch.randn(Dn, generator=g, device=DEV) * 0.1
+    ops.raw_oob_count()
+    if fused:
+        Wf = torch.full((V, ops.fused_slot(D)), 123.0, device=DEV)
+        Wf[:, :D] = W
+        Wf[:, D] = W1[:, 0]
+        feat, y1, y2, S = ops.raw_embed_fm_fwd(Wf, None, ids, dense, dense_w, dense_w1, 0, D=D)
+        del Wf
+    else:
+        feat, y1, y2, S = ops.raw_embed_fm_fwd(W, W1, ids, dense, dense_w, dense_w1, 0)
+    live = (ids != 0).unsqueeze(2)
+    assert torch.equal(feat[:, :F], W[ids] * live)
+    assert torch.equal(feat[:, F:], dense.unsqueeze(2) * dense_w.unsqueeze(0))
+    assert ops.raw_oob_count() == 0
+    f = feat.double()
+    assert_within(S, f.sum(1), N * U * f.abs().sum(1), "S")
+    t1 = torch.cat([(W1[ids, 0] * (ids != 0)).double(), dense.double() * dense_w1.double()], 1)
+    assert_within(y1, t1.sum(1), (N + 2) * U * t1.abs().sum(1), "y1")
+    Sd, Q = f.sum(1), f.square().sum(1)
+    A = f.abs().sum(1)
+    assert_within(y2, 0.5 * (Sd.square() - Q).sum(1),
+                  (4 * N + 2 * D + 8) * U * 0.5 * (A.square() + Q).sum(1), "y2")
+
+
+# ================================================================================================
+# 10. hash_keys and cvm (grid-stride over 16*SM CTAs of 256 threads)
+# ================================================================================================
+def test_hash_keys_at_scale():
+    """n = 4M keys: every thread folds >= 3 keys.  Bit-exact against oracle/readers.hash_keys."""
+    from oracle import readers
+    ops = _ops()
+    n = 4 << 20
+    assert_loops("hash_keys_kernel: keys per thread", n // (STREAM_CTAS_PER_SM * _sm() * 256))
+    rng = np.random.default_rng(4)
+    keys = rng.integers(0, 1 << 63, n, dtype=np.uint64) * np.uint64(2) + rng.integers(0, 2, n, dtype=np.uint64)
+    keys[::1000] = 0
+    slots = rng.integers(0, 26, n).astype(np.int32)
+    kd = torch.from_numpy(keys).to(DEV)
+    for V, sl, rz in ((1_000_003, slots, True), ((1 << 40) + 7, None, False)):
+        got = ops.raw_hash_keys(kd, V, None if sl is None else torch.from_numpy(sl).to(DEV), rz)
+        assert np.array_equal(got.cpu().numpy(), readers.hash_keys(keys, V, sl, rz))
+
+
+@pytest.mark.parametrize("use_cvm", [False, True])
+def test_cvm_at_scale(use_cvm):
+    """N = 1.7M rows of D+2 = 13: every thread handles >= 3 elements.  Copies are bit-exact; the
+    two log columns: logf(x + 1) is within 1 ulp after one rounded add, so each is within
+    2u(1 + |log|) and their difference within 4u(1 + |log(x0+1)| + |log(x1+1)|)."""
+    ops = _ops()
+    N, D = 1_700_000, 11
+    out_w = D + 2 if use_cvm else D
+    assert_loops("cvm_fwd_kernel: elements per thread", N * out_w // (STREAM_CTAS_PER_SM * _sm() * 256))
+    g = torch.Generator(device=DEV).manual_seed(11)
+    x = torch.rand(N, D + 2, generator=g, device=DEV) * 5
+    y = ops.raw_cvm_fwd(x, use_cvm)
+    assert torch.equal(y[:, -D:], x[:, 2:])
+    if use_cvm:
+        ref = nets.cvm(x.double(), True)
+        l0, l1 = torch.log1p(x[:, 0].double()), torch.log1p(x[:, 1].double())
+        bound = (4 * U * (1 + l0.abs() + l1.abs())).unsqueeze(1).expand(N, 2)
+        assert_within(y[:, :2], ref[:, :2], bound, "cvm log columns")
+    sc = torch.rand(N, 2, generator=g, device=DEV) * 3
+    dy = torch.randn(N, out_w, generator=g, device=DEV)
+    assert_loops("cvm_bwd_kernel: elements per thread", N * (D + 2) // (STREAM_CTAS_PER_SM * _sm() * 256))
+    dx = ops.raw_cvm_bwd(dy, sc, D, use_cvm)
+    assert torch.equal(dx[:, :2], sc) and torch.equal(dx[:, 2:], dy[:, -D:])
