@@ -189,7 +189,9 @@ int b200rec_din_attn_fwd(const float* hist, const float* tseq, const float* tb, 
  * memory; `peer_ptrs_host[r]` = base of rank r's buffer in THIS process's address space) and the
  * kernels store straight into them over NVLink.  seg_dev [world+1] / dst_dev [world] are DEVICE
  * int64 tables (outputs of the count exchange): rows [seg[r], seg[r+1]) of the local list go to
- * peer r, starting at row dst[r] of its buffer (row pitch ld_dst floats).
+ * peer r, starting at row dst[r] of its buffer (row pitch ld_dst floats).  The first `world`
+ * peer pointers must be non-null and aligned to the row store width (4*VEC bytes, VEC as for D;
+ * 16 bytes for shard_fm_grads_push), else B200REC_ERR_INVALID, checked also when n == 0.
  *   shard_gather_push  owner side of the pull: gather of the requested rows of `shard` (ids are
  *                      LOCAL rows; local_pad / out-of-range -> zeros) fused with their transfer
  *   shard_push_rows    requester side of the push: per-slot gradient rows (bucket order) -> owners

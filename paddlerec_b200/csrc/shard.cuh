@@ -269,8 +269,15 @@ static int launch_shard_fm_grads_push(const float* feat, const float* S, const f
                                       const uint64_t* peer_ptrs_host, int64_t ld_dst, int world,
                                       int64_t B, int F, int Dn, int D, int G, cudaStream_t st);
 
-static int fill_peer_table(PeerTable* t, const uint64_t* peer_ptrs_host, int world) {
+// align_bytes = width of the launcher's vector store: every peer base must allow it (the row pitch
+// is checked by the launcher), or the first store into that peer faults.
+static int fill_peer_table(PeerTable* t, const uint64_t* peer_ptrs_host, int world, int align_bytes) {
   B200_REQUIRE(world >= 1 && world <= kMaxPeers, "shard push: world=%d (max %d)", world, kMaxPeers);
+  for (int r = 0; r < world; ++r) {
+    B200_REQUIRE(peer_ptrs_host[r] != 0, "shard push: peer %d buffer is null", r);
+    B200_REQUIRE(peer_ptrs_host[r] % (uint64_t)align_bytes == 0,
+                 "shard push: peer %d buffer must be %d-byte aligned", r, align_bytes);
+  }
   for (int r = 0; r < kMaxPeers; ++r)
     t->base[r] = r < world ? reinterpret_cast<float*>((uintptr_t)peer_ptrs_host[r]) : nullptr;
   return B200REC_OK;
@@ -280,11 +287,11 @@ static int launch_shard_gather_push(const float* W, int64_t ldw, int D, int64_t 
                                     const int64_t* ids, const int64_t* seg_dev,
                                     const int64_t* dst_dev, const uint64_t* peer_ptrs_host,
                                     int64_t ld_dst, int world, int64_t n, cudaStream_t st) {
-  PeerTable t;
-  int rc = fill_peer_table(&t, peer_ptrs_host, world);
-  if (rc != B200REC_OK) return rc;
   RowShape rs;
   B200_REQUIRE(pick_row_shape(D, &rs), "shard_gather_push: unsupported D=%d", D);
+  PeerTable t;
+  int rc = fill_peer_table(&t, peer_ptrs_host, world, rs.vec * 4);
+  if (rc != B200REC_OK) return rc;
   B200_REQUIRE(ldw >= D && ld_dst >= D && ldw % rs.vec == 0 && ld_dst % rs.vec == 0,
                "shard_gather_push: bad row strides");
   B200_REQUIRE(reinterpret_cast<uintptr_t>(W) % (rs.vec * 4) == 0,
@@ -309,11 +316,11 @@ static int launch_shard_gather_push(const float* W, int64_t ldw, int D, int64_t 
 static int launch_shard_push_rows(const float* rows, int64_t ld, int D, const int64_t* seg_dev,
                                   const int64_t* dst_dev, const uint64_t* peer_ptrs_host,
                                   int64_t ld_dst, int world, int64_t n, cudaStream_t st) {
-  PeerTable t;
-  int rc = fill_peer_table(&t, peer_ptrs_host, world);
-  if (rc != B200REC_OK) return rc;
   RowShape rs;
   B200_REQUIRE(pick_row_shape(D, &rs), "shard_push_rows: unsupported D=%d", D);
+  PeerTable t;
+  int rc = fill_peer_table(&t, peer_ptrs_host, world, rs.vec * 4);
+  if (rc != B200REC_OK) return rc;
   B200_REQUIRE(ld >= D && ld_dst >= D && ld % rs.vec == 0 && ld_dst % rs.vec == 0,
                "shard_push_rows: bad row strides");
   B200_REQUIRE(reinterpret_cast<uintptr_t>(rows) % (rs.vec * 4) == 0,
@@ -341,7 +348,7 @@ static int launch_shard_fm_grads_push(const float* feat, const float* S, const f
                                       const uint64_t* peer_ptrs_host, int64_t ld_dst, int world,
                                       int64_t B, int F, int Dn, int D, int G, cudaStream_t st) {
   PeerTable t;
-  int rc = fill_peer_table(&t, peer_ptrs_host, world);
+  int rc = fill_peer_table(&t, peer_ptrs_host, world, 16);
   if (rc != B200REC_OK) return rc;
   B200_REQUIRE(D > 0 && D % 4 == 0 && G % 4 == 0 && G >= D + 1 && ld_dst >= G && ld_dst % 4 == 0,
                "shard_fm_grads_push: needs D %% 4 == 0 and G %% 4 == 0, G >= D+1 (D=%d G=%d)", D, G);

@@ -93,8 +93,9 @@ class PeerBuffers:
 
 
 P2P_MAX_WORLD = 4
-# b200rec_shard_fm_grads_push (K2's sparse half + the push as one kernel): compiled and desk-checked
-# but NOT yet run on a GPU (the round's GPU budget ended first) -> opt-in only.
+# b200rec_shard_fm_grads_push (K2's sparse half + the push as one kernel): opt-in.  On one H100 with
+# 2 to 8 virtual ranks it stores the same bits as K2 + shard_push_rows
+# (tests/test_gpu_shard_exchange.py), but it has not yet run across GPUs or been timed.
 FUSED_PUSH = os.environ.get("B200REC_FUSED_PUSH", "0") == "1"
 
 

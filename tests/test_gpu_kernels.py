@@ -249,19 +249,36 @@ def test_cross_v2(C):
     assert rel_err(dbias.cpu(), (dout.double() * x0.double()).sum(0)) < 2e-6
 
 
-@pytest.mark.parametrize("world", [1, 2, 8])
-def test_shard_bucketize(world):
+@pytest.mark.parametrize("world,n,only_owner", [
+    pytest.param(1, 5000, None, id="1"),
+    pytest.param(2, 5000, None, id="2"),
+    pytest.param(8, 5000, None, id="8"),
+    # the radix sort runs over ceil(log2(world)) bits (shard.cuh:54-55): not log2(world) for 3 and 5
+    pytest.param(3, 5000, None, id="3"),
+    pytest.param(5, 5000, None, id="5"),
+    pytest.param(16, 5000, None, id="16"),
+    pytest.param(4, 0, None, id="4-empty"),
+    pytest.param(5, 5000, 3, id="5-one-owner"),
+    pytest.param(16, 1_700_000, None, id="16-1.7M"),
+])
+def test_shard_bucketize(world, n, only_owner):
     ops = _ops()
-    V, n = 1000, 5000
-    g = torch.Generator().manual_seed(world)
-    ids = torch.randint(0, V, (n,), generator=g)
-    ids[10] = -5
-    ids[11] = V + 1
+    V = 1000
+    g = torch.Generator().manual_seed(world + n)
+    if only_owner is None:
+        ids = torch.randint(0, V, (n,), generator=g)
+        if n > 11:
+            ids[10] = -5
+            ids[11] = V + 1
+    else:
+        ids = torch.randint(0, V // world, (n,), generator=g) * world + only_owner
     send, perm, inv, counts = ops.raw_shard_bucketize(ids.to(DEV), world, V)
     send, perm, inv, counts = send.cpu(), perm.cpu(), inv.cpu().long(), counts.cpu()
     valid = (ids >= 0) & (ids < V)
     owner = torch.where(valid, ids % world, torch.zeros_like(ids))
     assert counts.tolist() == [int((owner == r).sum()) for r in range(world)]
+    if only_owner is not None:
+        assert counts.tolist() == [n if r == only_owner else 0 for r in range(world)]
     assert torch.equal(perm[inv], torch.arange(n))            # inverse permutations
     assert (owner[inv][1:] >= owner[inv][:-1]).all()          # bucket order is owner-major
     off = 0

@@ -461,8 +461,10 @@ def _peer_worker(rank, world, port, out_dir, bufs, cap, fused_push):
 def test_peer_memory_choreography_on_host_buffers(world, fused_push, tmp_path):
     """The peer-memory pull / push of ShardExchange (and, with fused_push, the one-kernel
     FM-gradient push) replayed on shared host tensors: same oracle, same tolerances as the all-to-all
-    path.  Covers the host logic (tables, buffer offsets, barriers, zero-segment K2 call); the CUDA
-    kernels themselves are covered by tests/test_sharded_gpu.py."""
+    path.  Covers the host logic (tables, buffer offsets, barriers, zero-segment K2 call).  The CUDA
+    kernels themselves are covered on one GPU by tests/test_gpu_shard_exchange.py (virtual ranks
+    whose receive buffers share one device tensor, worlds 1 to 16) and on 2+ GPUs by
+    tests/test_sharded_gpu.py."""
     B = _batch_for(world)
     cols = (D + 1 + 3) // 4 * 4
     cap = B // world * F + 8
