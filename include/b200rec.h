@@ -312,8 +312,8 @@ int b200rec_log_loss_mean_bwd(const float* pred, const void* label, int label_is
 int b200rec_auc_update(const float* pred, const void* label, int label_is_i64, int64_t* stat_pos,
                        int64_t* stat_neg, int num_thresholds, int64_t n, void* stream);
 /* tuning / bring-up knobs (key 0: force tile width BN; 1-3: descriptor overrides of the dW kernel;
- * 4: k-block of the K-major kernel, 64 = 128-byte swizzle, 32 = 64-byte swizzle, more stages)
- * and the device word a pipeline watchdog writes before it traps. */
+ * 4: k-block of the K-major kernel, 32 = 64-byte swizzle (the default), 64 = 128-byte swizzle,
+ * fewer stages) and the device word a pipeline watchdog writes before it traps. */
 int b200rec_tc_debug(int key, int value);
 int b200rec_tc_timeout_word(unsigned int* word_host);
 

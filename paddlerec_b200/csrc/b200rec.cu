@@ -536,7 +536,7 @@ int b200rec_tc_debug(int key, int value) {
     case 1: tc::g_dw_debug.lbo_a = (uint32_t)value; break;
     case 2: tc::g_dw_debug.lbo_b = (uint32_t)value; break;
     case 3: tc::g_dw_debug.sbo = (uint32_t)value; break;
-    case 4: tc::g_bk = value == 32 ? 32 : 64; break;
+    case 4: tc::g_bk = value == 64 ? 64 : 32; break;
     default: set_error("tc_debug: unknown key %d", key); return B200REC_ERR_INVALID;
   }
   return B200REC_OK;

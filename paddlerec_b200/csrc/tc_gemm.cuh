@@ -17,9 +17,10 @@
 //   tc_gemm_kmajor_kernel   D[M,N] = A[M,K] . B[N,K]^T     both operands K-major (reduction dim
 //       contiguous): forward (A = activations, B = W^T planes) and dX (A = dZ planes, B = W
 //       planes).  Persistent over 128 x BN output tiles; the producer streams the next tile's
-//       k-blocks while the consumers run the epilogue of the current one.  Fused epilogues, straight
-//       from the accumulator registers: +bias, ReLU, hi/lo split (emits the NEXT GEMM's operand
-//       directly), ReLU mask + bias column-sum in backward, or plain fp32.
+//       k-blocks while the consumers run the epilogue of the current one.  Fused epilogues, staged
+//       through shared memory per warp and stored row-contiguously: +bias, ReLU, hi/lo split (emits
+//       the NEXT GEMM's operand directly), ReLU mask + bias column-sum in backward, CrossNet, or
+//       plain fp32.
 //   tc_gemm_dw_kernel       dW[K,N] = sum_m A[m,K] . G[m,N]   both operands MN-major (the batch dim
 //       is the reduction; wgmma reads both transposed), split over the batch across CTAs, fp32
 //       partial tiles + fixed-order reduce (deterministic, no atomics).
@@ -30,6 +31,8 @@
 
 #include <cuda.h>  // CUtensorMap and enums only; cuTensorMapEncodeTiled is resolved at run time
 #include <cuda_bf16.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -100,6 +103,15 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, 
       " [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
       "l"(m), "r"(bar), "r"(x), "r"(y)
       : "memory");
+}
+// move registers from the producer warpgroup to the consumers (all 128 threads of a warpgroup)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -299,6 +311,15 @@ struct Epilogue {
   int64_t ld_add;
   float* aux_f32;                   // [M, ld_aux] receives acc + bias + addend, i.e. the value BEFORE
   int64_t ld_aux;                   //   the CrossNet / ReLU / mask transforms, or null
+  // filled in by launch_gemm_kmajor, not by the callers:
+  int vec;                          // kVec* bits: the operand allows one 16-byte (fp32) or 8-byte
+                                    //   (bf16) access per 4 columns at every row
+  int extra;                        // addend, aux_f32 or CrossNet in use (the second epilogue body)
+};
+
+enum : int {
+  kVecBias = 1, kVecF32 = 2, kVecPlanes = 4, kVecMask = 8, kVecAdd = 16, kVecAux = 32,
+  kVecCross = 64,
 };
 
 __device__ __forceinline__ void split_bf16(float x, float& hi_f, __nv_bfloat16& hi,
@@ -318,18 +339,7 @@ __device__ __forceinline__ void split_pack2(float a, float b, uint32_t& hi, uint
 }
 
 __device__ __forceinline__ bool al8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
-__device__ __forceinline__ bool al4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3u) == 0; }
 
-// p[0], p[1] (the second only if `two`): one 64-bit access where the address allows it
-__device__ __forceinline__ void ld_pair(const float* p, bool two, float& x, float& y) {
-  if (two && al8(p)) {
-    const float2 v = __ldg(reinterpret_cast<const float2*>(p));
-    x = v.x; y = v.y;
-  } else {
-    x = __ldg(p);
-    y = two ? __ldg(p + 1) : 0.f;
-  }
-}
 __device__ __forceinline__ void st_pair(float* p, bool two, float x, float y) {
   if (two && al8(p)) {
     *reinterpret_cast<float2*>(p) = make_float2(x, y);
@@ -338,108 +348,220 @@ __device__ __forceinline__ void st_pair(float* p, bool two, float x, float y) {
     if (two) p[1] = y;
   }
 }
-__device__ __forceinline__ void st_pair_bf16(__nv_bfloat16* p, bool two, uint32_t packed) {
-  if (two && al4(p)) {
-    *reinterpret_cast<uint32_t*>(p) = packed;
-  } else {
-    p[0] = __ushort_as_bfloat16((unsigned short)(packed & 0xFFFFu));
-    if (two) p[1] = __ushort_as_bfloat16((unsigned short)(packed >> 16));
+
+// p[0 .. n), n in 1..4, as one access where `vec` allows it; missing elements read as 0
+__device__ __forceinline__ float4 ld4(const float* p, int n, bool vec) {
+  if (vec && n == 4) return __ldg(reinterpret_cast<const float4*>(p));
+  float4 v = make_float4(__ldg(p), 0.f, 0.f, 0.f);
+  if (n > 1) v.y = __ldg(p + 1);
+  if (n > 2) v.z = __ldg(p + 2);
+  if (n > 3) v.w = __ldg(p + 3);
+  return v;
+}
+__device__ __forceinline__ void st4(float* p, int n, bool vec, float4 v) {
+  if (vec && n == 4) {
+    *reinterpret_cast<float4*>(p) = v;
+    return;
   }
+  p[0] = v.x;
+  if (n > 1) p[1] = v.y;
+  if (n > 2) p[2] = v.z;
+  if (n > 3) p[3] = v.w;
+}
+// four bf16 packed in two 32-bit words (element 0 in the low half of w.x)
+__device__ __forceinline__ uint2 ld4_bf16(const __nv_bfloat16* p, int n, bool vec) {
+  if (vec && n == 4) return __ldg(reinterpret_cast<const uint2*>(p));
+  const unsigned short* q = reinterpret_cast<const unsigned short*>(p);
+  uint2 w = make_uint2(__ldg(q), 0u);
+  if (n > 1) w.x |= (uint32_t)__ldg(q + 1) << 16;
+  if (n > 2) w.y = __ldg(q + 2);
+  if (n > 3) w.y |= (uint32_t)__ldg(q + 3) << 16;
+  return w;
+}
+__device__ __forceinline__ void st4_bf16(__nv_bfloat16* p, int n, bool vec, uint2 w) {
+  if (vec && n == 4) {
+    *reinterpret_cast<uint2*>(p) = w;
+    return;
+  }
+  unsigned short* q = reinterpret_cast<unsigned short*>(p);
+  q[0] = (unsigned short)(w.x & 0xFFFFu);
+  if (n > 1) q[1] = (unsigned short)(w.x >> 16);
+  if (n > 2) q[2] = (unsigned short)(w.y & 0xFFFFu);
+  if (n > 3) q[3] = (unsigned short)(w.y >> 16);
 }
 
-// The two horizontally adjacent accumulator values (row, col) and (row, col + 1) of one thread ->
-// outputs; returns the emitted values.  `two`: column col + 1 exists in the matrix (else b is
-// dropped and returned as 0, so that column sums stay exact).  The caller skips rows outside the
-// matrix.  Not inlined on purpose: the tile epilogue calls it BN / 4 times per thread, and inlined
-// copies of this body for a 256-wide tile outgrow the instruction cache (measured: the K-major
-// GEMM at BN = 256 ran at a fifth of the dW kernel's rate).
-__device__ __noinline__ float2 epilogue_pair(const Epilogue& ep, float a, float b, int64_t row,
-                                             int col, bool two) {
-  float x, y;
-  if (ep.bias != nullptr) {
-    ld_pair(ep.bias + col, two, x, y);
-    a += x; b += y;
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+  asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+}
+// the 128-byte lines of `bytes` bytes at p, spread over the two lanes (lane & 1) of a row
+__device__ __forceinline__ void prefetch_row_l2(const void* p, int bytes, int lane) {
+  const uintptr_t a0 = reinterpret_cast<uintptr_t>(p) & ~(uintptr_t)127;
+  const uintptr_t a1 = reinterpret_cast<uintptr_t>(p) + (uintptr_t)bytes - 1;
+  for (uintptr_t a = a0 + 128u * (uintptr_t)(lane & 1); a <= a1; a += 256u)
+    prefetch_l2(reinterpret_cast<const void*>(a));
+}
+
+// Epilogue staging: each consumer warp passes its 16 x BN accumulator rows through shared memory
+// in chunks of 16 rows x 32 columns (fp32, rows padded to 40 floats: the fragment's float2 writes
+// and the row-contiguous float4 reads are both free of bank conflicts).  Read back row-contiguously,
+// every global access of a quarter-warp covers one row segment of 4 x 8 columns: 128-byte fp32
+// stores, 64-byte stores into each bf16 plane.
+constexpr int kEpCols = 32;
+constexpr int kEpPitch = 40;
+constexpr uint32_t kEpWarpFloats = 16u * kEpPitch;
+constexpr uint32_t kEpSmemBytes = kConsumerWarps * kEpWarpFloats * 4u;
+
+// Accumulator fragment columns [32 c, 32 c + 32) -> the warp's staging chunk (wgmma layout: the
+// thread holds rows lane / 4 and + 8, columns 8 j + 2 (lane % 4) + {0, 1}).  The chunk index is a
+// run-time value; the accumulator registers are selected by a chain of compile-time cases.
+template <int BN, int C = 0>
+__device__ __forceinline__ void stage_chunk(const float (&acc)[BN / 2], float* stg, int c, int lane) {
+  if (c == C) {
+    constexpr int CW = BN - kEpCols * C < kEpCols ? BN - kEpCols * C : kEpCols;
+    constexpr int j0 = kEpCols / 8 * C;
+    const int lc = 2 * (lane & 3), rr = lane >> 2;
+#pragma unroll
+    for (int jj = 0; jj < CW / 8; ++jj) {
+      *reinterpret_cast<float2*>(stg + rr * kEpPitch + 8 * jj + lc) =
+          make_float2(acc[4 * (j0 + jj)], acc[4 * (j0 + jj) + 1]);
+      *reinterpret_cast<float2*>(stg + (rr + 8) * kEpPitch + 8 * jj + lc) =
+          make_float2(acc[4 * (j0 + jj) + 2], acc[4 * (j0 + jj) + 3]);
+    }
+    return;
   }
-  if (ep.addend != nullptr) {
-    ld_pair(ep.addend + row * ep.ld_add + col, two, x, y);
-    a += x; b += y;
-  }
-  if (ep.aux_f32 != nullptr) st_pair(ep.aux_f32 + row * ep.ld_aux + col, two, a, b);
-  if (ep.cross_x0 != nullptr) {
-    float z, w;
-    ld_pair(ep.cross_x0 + row * ep.ld_cross + col, two, x, y);
-    ld_pair(ep.cross_xl + row * ep.ld_cross + col, two, z, w);
-    a = fmaf(x, a, z);
-    b = fmaf(y, b, w);
-  }
-  if (ep.relu) {
-    a = fmaxf(a, 0.f);
-    b = fmaxf(b, 0.f);
-  }
+  if constexpr (kEpCols * (C + 1) < BN) stage_chunk<BN, C + 1>(acc, stg, c, lane);
+}
+
+// One chunk of a consumer warp's epilogue: matrix columns [c0, c0 + cw) of the warp's 16 rows (first
+// row r0).  Lane l handles columns c0 + 4 (l % 8) .. + 3 in rows l / 8 + 4 p, p = 0..3.  The side
+// inputs of the chunk are loaded first, then stage() puts the raw accumulators into `stg`.  The
+// transforms apply in this order: + bias, + addend, aux store, CrossNet fma, ReLU, mask, then the
+// fp32 and hi/lo stores, the same per-element arithmetic as an unstaged epilogue.  kExtra: the
+// addend / aux / CrossNet body; without it those fields are ignored.  With s_cs (the warp's column
+// sums of this chunk) the emitted values are summed over the warp's rows in a fixed order.
+template <bool kExtra, typename Stage>
+__device__ __forceinline__ void epilogue_rows(const Epilogue& ep, const float* stg, int M, int N,
+                                              int64_t r0, int c0, int cw, int lane, float* s_cs,
+                                              Stage stage) {
+  const int g = lane & 7, lr = lane >> 3;
+  const int col = c0 + 4 * g;
+  int n = 4 * g < cw ? N - col : 0;           // valid columns of this lane (<= 0: none)
+  n = n > 4 ? 4 : n;
+  const int vec = ep.vec;
+
+  float4 bias = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (ep.bias != nullptr && n > 0) bias = ld4(ep.bias + col, n, vec & kVecBias);
+  uint2 mw[4];
   if (ep.mask_src != nullptr) {
-    const __nv_bfloat16* m = ep.mask_src + row * ep.ld_mask + col;
-    // bf16 > 0  <=>  its bit pattern, as a signed integer in the high half, is > 0
-    uint32_t w;
-    if (two && al4(m))
-      w = __ldg(reinterpret_cast<const unsigned int*>(m));
-    else
-      w = (uint32_t)__bfloat16_as_ushort(m[0]) |
-          (two ? (uint32_t)__bfloat16_as_ushort(m[1]) << 16 : 0u);
-    if (!((int)(w << 16) > 0)) a = 0.f;
-    if (!((int)(w & 0xFFFF0000u) > 0)) b = 0.f;
-  }
-  if (!two) b = 0.f;
-  if (ep.out_f32 != nullptr) st_pair(ep.out_f32 + row * ep.ld_f32 + col, two, a, b);
-  if (ep.out_planes != nullptr) {
-    __nv_bfloat16* oh = ep.out_planes + row * 2 * ep.ldp + col;
-    uint32_t h, l;
-    split_pack2(a, b, h, l);
-    st_pair_bf16(oh, two, h);
-    st_pair_bf16(oh + ep.ldp, two, l);
-  }
-  return make_float2(a, b);
-}
-
-// One consumer thread's share of a 128 x BN accumulator tile -> outputs.  wgmma m64nN layout: the
-// thread holds rows r0 = 16 * (warp in warpgroup) + lane / 4 and r0 + 8 of its warpgroup's 64 rows,
-// columns 8 j + 2 (lane % 4) + {0, 1}: acc[4j], acc[4j + 1] on row r0, acc[4j + 2], acc[4j + 3] on
-// row r0 + 8.  With s_colsum ([8 consumer warps][kMaxBN]) the warp's column sums of the emitted
-// values land there (fixed-order shuffle tree: deterministic).
-template <int BN>
-__device__ __forceinline__ void epilogue_tile(const Epilogue& ep, float (&acc)[BN / 2], int M,
-                                              int N, int m0, int n0, int cw, int lane,
-                                              float* s_colsum) {
-  const int64_t r0 = (int64_t)m0 + 16 * cw + (lane >> 2);
-  const bool ok0 = r0 < M, ok1 = r0 + 8 < M;
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int col = n0 + 8 * j + 2 * (lane & 3);
-    const bool in = col < N, two = col + 1 < N;
-    float2 v0 = make_float2(0.f, 0.f), v1 = make_float2(0.f, 0.f);
-    if (in && ok0) v0 = epilogue_pair(ep, acc[4 * j], acc[4 * j + 1], r0, col, two);
-    if (in && ok1) v1 = epilogue_pair(ep, acc[4 * j + 2], acc[4 * j + 3], r0 + 8, col, two);
-    acc[4 * j] = v0.x; acc[4 * j + 1] = v0.y; acc[4 * j + 2] = v1.x; acc[4 * j + 3] = v1.y;
-    if (s_colsum != nullptr) {
-      float s0 = acc[4 * j] + acc[4 * j + 2], s1 = acc[4 * j + 1] + acc[4 * j + 3];
-#pragma unroll
-      for (int h = 4; h <= 16; h <<= 1) {
-        s0 += __shfl_xor_sync(0xffffffffu, s0, h);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, h);
-      }
-      if (lane < 4) {
-        s_colsum[8 * j + 2 * lane] = s0;
-        s_colsum[8 * j + 2 * lane + 1] = s1;
-      }
+    for (int p = 0; p < 4; ++p) {
+      const int64_t row = r0 + lr + 4 * p;
+      mw[p] = n > 0 && row < M ? ld4_bf16(ep.mask_src + row * ep.ld_mask + col, n, vec & kVecMask)
+                               : make_uint2(0u, 0u);
     }
   }
-  if (ep.ones_col && ep.out_planes != nullptr && (lane & 3) == 0 && n0 + BN >= N) {
-    for (int h = 0; h < 2; ++h) {
-      const int64_t row = r0 + 8 * h;
-      if (row < M) {
-        __nv_bfloat16* oh = ep.out_planes + row * 2 * ep.ldp + N;
-        oh[0] = __float2bfloat16_rn(1.f);
-        oh[ep.ldp] = __float2bfloat16_rn(0.f);
+  __syncwarp();                                // the previous chunk's reads are done
+  stage();
+  __syncwarp();
+
+  float4 cs = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+  for (int p = 0; p < 4; ++p) {
+    const int64_t row = r0 + lr + 4 * p;
+    if (n <= 0 || row >= M) continue;
+    float4 v = *reinterpret_cast<const float4*>(stg + (lr + 4 * p) * kEpPitch + 4 * g);
+    if (ep.bias != nullptr) {
+      v.x += bias.x; v.y += bias.y; v.z += bias.z; v.w += bias.w;
+    }
+    if (kExtra) {
+      if (ep.addend != nullptr) {
+        const float4 a = ld4(ep.addend + row * ep.ld_add + col, n, vec & kVecAdd);
+        v.x += a.x; v.y += a.y; v.z += a.z; v.w += a.w;
       }
+      if (ep.aux_f32 != nullptr) st4(ep.aux_f32 + row * ep.ld_aux + col, n, vec & kVecAux, v);
+      if (ep.cross_x0 != nullptr) {
+        const float4 x0 = ld4(ep.cross_x0 + row * ep.ld_cross + col, n, vec & kVecCross);
+        const float4 xl = ld4(ep.cross_xl + row * ep.ld_cross + col, n, vec & kVecCross);
+        v.x = fmaf(x0.x, v.x, xl.x); v.y = fmaf(x0.y, v.y, xl.y);
+        v.z = fmaf(x0.z, v.z, xl.z); v.w = fmaf(x0.w, v.w, xl.w);
+      }
+    }
+    if (ep.relu) {
+      v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
+    }
+    if (ep.mask_src != nullptr) {
+      // bf16 > 0  <=>  its bit pattern, as a signed integer in the high half, is > 0
+      if (!((int)(mw[p].x << 16) > 0)) v.x = 0.f;
+      if (!((int)(mw[p].x & 0xFFFF0000u) > 0)) v.y = 0.f;
+      if (!((int)(mw[p].y << 16) > 0)) v.z = 0.f;
+      if (!((int)(mw[p].y & 0xFFFF0000u) > 0)) v.w = 0.f;
+    }
+    if (n < 4) {                               // columns past N: nothing stored, 0 in the sums
+      if (n < 2) v.y = 0.f;
+      if (n < 3) v.z = 0.f;
+      v.w = 0.f;
+    }
+    if (ep.out_f32 != nullptr) st4(ep.out_f32 + row * ep.ld_f32 + col, n, vec & kVecF32, v);
+    if (ep.out_planes != nullptr) {
+      __nv_bfloat16* oh = ep.out_planes + row * 2 * ep.ldp + col;
+      uint2 h, l;
+      split_pack2(v.x, v.y, h.x, l.x);
+      split_pack2(v.z, v.w, h.y, l.y);
+      st4_bf16(oh, n, vec & kVecPlanes, h);
+      st4_bf16(oh + ep.ldp, n, vec & kVecPlanes, l);
+    }
+    cs.x += v.x; cs.y += v.y; cs.z += v.z; cs.w += v.w;
+  }
+  if (s_cs != nullptr) {                       // fixed-order tree over the 4 lanes of a column group
+#pragma unroll
+    for (int h = 8; h <= 16; h <<= 1) {
+      cs.x += __shfl_xor_sync(0xffffffffu, cs.x, h);
+      cs.y += __shfl_xor_sync(0xffffffffu, cs.y, h);
+      cs.z += __shfl_xor_sync(0xffffffffu, cs.z, h);
+      cs.w += __shfl_xor_sync(0xffffffffu, cs.w, h);
+    }
+    if (lane < 8 && 4 * lane < cw) *reinterpret_cast<float4*>(s_cs + 4 * lane) = cs;
+  }
+}
+
+// One consumer warp's 16 x BN share of a 128 x BN accumulator tile -> outputs, in chunks of 32
+// columns.  r0: the warp's first matrix row.  With s_cs ([kMaxBN]) the warp's column sums of the
+// emitted values land there.  The chunk loop is not unrolled: one copy of each epilogue body.
+template <int BN>
+__device__ __forceinline__ void epilogue_tile(const Epilogue& ep, const float (&acc)[BN / 2],
+                                              float* stg, int M, int N, int64_t r0, int n0, int lane,
+                                              float* s_colsum) {
+  constexpr int kChunks = (BN + kEpCols - 1) / kEpCols;
+#pragma unroll 1
+  for (int c = 0; c < kChunks; ++c) {
+    const int cw = BN - kEpCols * c < kEpCols ? BN - kEpCols * c : kEpCols;
+    float* s_cs = s_colsum != nullptr ? s_colsum + kEpCols * c : nullptr;
+    auto stage = [&] { stage_chunk<BN>(acc, stg, c, lane); };
+    if (ep.extra)
+      epilogue_rows<true>(ep, stg, M, N, r0, n0 + kEpCols * c, cw, lane, s_cs, stage);
+    else
+      epilogue_rows<false>(ep, stg, M, N, r0, n0 + kEpCols * c, cw, lane, s_cs, stage);
+  }
+  if (ep.ones_col && ep.out_planes != nullptr && n0 + BN >= N && lane < 16 && r0 + lane < M) {
+    __nv_bfloat16* oh = ep.out_planes + (r0 + lane) * 2 * ep.ldp + N;
+    oh[0] = __float2bfloat16_rn(1.f);
+    oh[ep.ldp] = __float2bfloat16_rn(0.f);
+  }
+}
+
+// The side inputs a warp's epilogue will read for its 16 rows of a tile, fetched into L2 while the
+// tile's products run (the saved activations they come from are far larger than L2).
+__device__ __forceinline__ void epilogue_prefetch(const Epilogue& ep, int M, int N, int BN,
+                                                 int64_t r0, int n0, int lane) {
+  const int64_t row = r0 + (lane >> 1);
+  if (row >= M) return;
+  const int w = N - n0 < BN ? N - n0 : BN;
+  if (ep.mask_src != nullptr) prefetch_row_l2(ep.mask_src + row * ep.ld_mask + n0, 2 * w, lane);
+  if (ep.extra) {
+    if (ep.addend != nullptr) prefetch_row_l2(ep.addend + row * ep.ld_add + n0, 4 * w, lane);
+    if (ep.cross_x0 != nullptr) {
+      prefetch_row_l2(ep.cross_x0 + row * ep.ld_cross + n0, 4 * w, lane);
+      prefetch_row_l2(ep.cross_xl + row * ep.ld_cross + n0, 4 * w, lane);
     }
   }
 }
@@ -447,8 +569,10 @@ __device__ __forceinline__ void epilogue_tile(const Epilogue& ep, float (&acc)[B
 // ------------------------------------------------------------------------------------------------
 // K-major GEMM: D[M,N] = A[M,K] . B[N,K]^T  (three wgmma per 16-wide k step)
 //   BK = 64: 128-byte swizzle rows (2 pipeline stages at BN = 208)
-//   BK = 32: 64-byte swizzle rows, half-size stages -> 5 stages at BN = 208: same bytes in shared
-//            memory, but a freed slot is refilled twice as early, which hides the TMA latency
+//   BK = 32: 64-byte swizzle rows, half-size stages -> 4 stages at BN = 208: about the same bytes in
+//            shared memory, but a freed slot is refilled twice as early, which hides the TMA latency
+// The producer warpgroup hands registers to the consumers (setmaxnreg): a consumer thread holds
+// BN / 2 accumulators through the whole epilogue.
 // ------------------------------------------------------------------------------------------------
 template <int BN, int BK>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -467,15 +591,21 @@ tc_gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA_hi,
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;          // swizzled tiles: atom-aligned
   uint8_t* sm = smem_raw + (base - raw);
-  // [stages][full barriers][empty barriers][colsum scratch: 8 warps x kMaxBN]
+  // [stages][full barriers][empty barriers][colsum scratch: 8 warps x kMaxBN][epilogue staging]
   const uint32_t bar_full = base + (uint32_t)stages * stage_bytes;
   const uint32_t bar_empty = bar_full + 8u * stages;
   float* s_colsum = reinterpret_cast<float*>(sm + (size_t)stages * stage_bytes + 16 * stages);
+  float* s_stage = s_colsum + kConsumerWarps * kMaxBN;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_m = (M + kBM - 1) / kBM, tiles_n = (N + BN - 1) / BN;
   const int n_tiles = tiles_m * tiles_n;
   const int nkb = (K + BK - 1) / BK;
+  // the consumers split the k-blocks into nfull blocks of BK / 16 real k-steps and, if tail > 0, a
+  // last block of tail < BK / 16 steps
+  const int last_steps = (K - (nkb - 1) * BK + kUK - 1) / kUK;
+  const int tail = last_steps == BK / kUK ? 0 : last_steps;
+  const int nfull = tail ? nkb - 1 : nkb;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA_hi); prefetch_tmap(&tmA_lo); prefetch_tmap(&tmB_hi); prefetch_tmap(&tmB_lo);
@@ -488,6 +618,7 @@ tc_gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA_hi,
   __syncthreads();
 
   if (warp < 4) {
+    setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -507,23 +638,28 @@ tc_gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA_hi,
       }
     }
   } else {
+    setmaxnreg_inc<232>();            // 128 x 40 + 256 x 232 registers <= 64 K
     const int cw = warp - 4;          // consumer warp 0..7; warpgroup = cw / 4 owns rows 64 (cw / 4)..
     const int wg = cw >> 2;
     const bool want_colsum = ep.colsum != nullptr;
+    float* const stg = s_stage + cw * kEpWarpFloats;
     float acc[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       const int m_blk = tile / tiles_n;
       const int m0 = m_blk * kBM, n0 = (tile % tiles_n) * BN;
+      const int64_t r0 = (int64_t)m0 + 64 * wg + 16 * (cw & 3);   // this warp's first row
+      epilogue_prefetch(ep, M, N, BN, r0, n0, lane);
       int prev = 0;
-      for (int kb = 0; kb < nkb; ++kb) {
+      // one k-block of NS 16-wide k-steps: three wgmma per step, one commit group per block
+      auto kblock = [&](auto ns, int kb) {
         mbar_wait(bar_full + 8u * stage, phase, 0x300u + stage);
         const uint32_t sA = base + (uint32_t)stage * stage_bytes + (uint32_t)wg * (64u * kRow);
         const uint32_t sB = base + (uint32_t)stage * stage_bytes + 2u * a_bytes;
         wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < BK / kUK; ++j) {
+        for (int j = 0; j < decltype(ns)::value; ++j) {
           const uint32_t ko = (uint32_t)j * (kUK * 2);   // 32 bytes further inside the swizzle row
           const uint64_t a_hi = gmma_desc(sA + ko, 16, kSbo, kLayout);
           const uint64_t a_lo = gmma_desc(sA + a_bytes + ko, 16, kSbo, kLayout);
@@ -540,11 +676,21 @@ tc_gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA_hi,
         }
         prev = stage;
         if (++stage == stages) { stage = 0; phase ^= 1u; }
-      }
+      };
+      constexpr int kSteps = BK / kUK;
+      for (int kb = 0; kb < nfull; ++kb) kblock(std::integral_constant<int, kSteps>(), kb);
+      // A last block with fewer real k-steps skips the steps that would multiply TMA's zero fill.
+      // Each tail length runs as a loop of 0 or 1 trips, not as a branch: wgmma issued inside a
+      // conditional path is serialized by ptxas.
+      for (int t = 0; t < (tail == 1); ++t) kblock(std::integral_constant<int, 1>(), nfull);
+      if constexpr (kSteps > 2)
+        for (int t = 0; t < (tail == 2); ++t) kblock(std::integral_constant<int, 2>(), nfull);
+      if constexpr (kSteps > 3)
+        for (int t = 0; t < (tail == 3); ++t) kblock(std::integral_constant<int, 3>(), nfull);
       wgmma_wait<0>();
       fence_acc(acc);
       if (lane == 0) mbar_arrive(bar_empty + 8u * prev);
-      epilogue_tile<BN>(ep, acc, M, N, m0 + 64 * wg, n0, cw & 3, lane,
+      epilogue_tile<BN>(ep, acc, stg, M, N, r0, n0, lane,
                         want_colsum ? s_colsum + cw * kMaxBN : nullptr);
       if (want_colsum) {
         named_bar_sync(1, 32 * kConsumerWarps);
@@ -808,7 +954,10 @@ static int make_map(CUtensorMap* m, const void* base, int64_t width, int64_t row
 
 static DwDebug g_dw_debug = {0u, 0u, 0u};
 static int g_bn_override = 0;
-static int g_bk = 64;   // k-block of the K-major kernel: 64 (SWIZZLE_128B) or 32 (SWIZZLE_64B)
+// k-block of the K-major kernel: 32 (SWIZZLE_64B, 4 stages at BN = 208) or 64 (SWIZZLE_128B, 2
+// stages).  At every forward and dX shape of the DeepFM tower 32 is faster or within 2 % of 64
+// (tools/tc_probe.py perf), so it is not chosen per shape.
+static int g_bk = 32;
 
 // Tile widths the K-major kernel is compiled for.  The choice minimises the padded output width
 // plus a per-tile charge of 64 columns for re-reading the A tile (N = 400 -> 2 x 208, 624 -> 3 x 208,
@@ -838,11 +987,12 @@ template <int BN, int BK>
 static int launch_kmajor_tiles(const CUtensorMap (&mp)[4], int64_t M, int N, int K,
                                const Epilogue& ep, cudaStream_t st) {
   constexpr uint32_t stage_bytes = (2u * kBM + 2u * BN) * (uint32_t)BK * 2u;
-  constexpr uint32_t fixed = kConsumerWarps * kMaxBN * 4u + 16u * 8u + 1024u;
+  constexpr uint32_t scratch = kConsumerWarps * kMaxBN * 4u + kEpSmemBytes;
+  constexpr uint32_t fixed = scratch + 16u * 8u + 1024u;
   int stages = (int)((kSmemBudget - fixed) / stage_bytes);
   stages = stages > 8 ? 8 : stages;
   B200_REQUIRE(stages >= 2, "tc_gemm: tile does not fit shared memory");
-  const size_t smem = (size_t)stages * stage_bytes + 16 * stages + kConsumerWarps * kMaxBN * 4 + 1024;
+  const size_t smem = (size_t)stages * stage_bytes + 16 * stages + scratch + 1024;
   static bool attr_set = false;
   if (!attr_set) {
     B200_CUDA(cudaFuncSetAttribute(tc_gemm_kmajor_kernel<BN, BK>,
@@ -870,13 +1020,28 @@ static int launch_kmajor_bk(int BN, const CUtensorMap (&mp)[4], int64_t M, int N
 }
 
 // D = A . B^T with A planes [M, 2*lda] (logical [M,K]) and B planes [N, 2*ldb] (logical [N,K]).
+// p is set, and 4 elements at any row and any column multiple of 4 are one `bytes`-aligned access
+static bool aligned_rows(const void* p, int64_t ld, unsigned bytes) {
+  return p != nullptr && reinterpret_cast<uintptr_t>(p) % bytes == 0 && ld % 4 == 0;
+}
+
 static int launch_gemm_kmajor(const void* A, int64_t lda, const void* B, int64_t ldb, int64_t M,
-                              int N, int K, const Epilogue& ep, cudaStream_t st) {
+                              int N, int K, const Epilogue& ep_in, cudaStream_t st) {
   B200_REQUIRE(M >= 0 && N > 0 && K > 0, "tc_gemm: bad sizes M=%lld N=%d K=%d", (long long)M, N, K);
   B200_REQUIRE(M < (1ll << 31), "tc_gemm: M too large");
   if (M == 0) return B200REC_OK;
+  Epilogue ep = ep_in;
+  ep.vec = (aligned_rows(ep.bias, 0, 16) ? kVecBias : 0) |
+           (aligned_rows(ep.out_f32, ep.ld_f32, 16) ? kVecF32 : 0) |
+           (aligned_rows(ep.out_planes, ep.ldp, 8) ? kVecPlanes : 0) |
+           (aligned_rows(ep.mask_src, ep.ld_mask, 8) ? kVecMask : 0) |
+           (aligned_rows(ep.addend, ep.ld_add, 16) ? kVecAdd : 0) |
+           (aligned_rows(ep.aux_f32, ep.ld_aux, 16) ? kVecAux : 0) |
+           (aligned_rows(ep.cross_x0, ep.ld_cross, 16) && aligned_rows(ep.cross_xl, ep.ld_cross, 16)
+                ? kVecCross : 0);
+  ep.extra = ep.addend != nullptr || ep.aux_f32 != nullptr || ep.cross_x0 != nullptr;
   const int BN = pick_bn(N);
-  const int BK = g_bk == 64 ? 64 : 32;
+  const int BK = g_bk;
   const __nv_bfloat16* a = static_cast<const __nv_bfloat16*>(A);
   const __nv_bfloat16* b = static_cast<const __nv_bfloat16*>(B);
   CUtensorMap mp[4];

@@ -24,18 +24,35 @@ def _join(planes, n):
     return p[:, :n] + p[:, ld:ld + n]
 
 
-def _time(fn, iters=10):
+def _time(fn, iters=10, warmup=1, repeats=1):
+    """ms per call: median over `repeats` windows of `iters` back-to-back calls, after `warmup`."""
     import torch
-    fn()
-    torch.cuda.synchronize()
-    t0 = torch.cuda.Event(enable_timing=True)
-    t1 = torch.cuda.Event(enable_timing=True)
-    t0.record()
-    for _ in range(iters):
+    for _ in range(warmup):
         fn()
-    t1.record()
     torch.cuda.synchronize()
-    return t0.elapsed_time(t1) / iters
+    ts = []
+    for _ in range(repeats):
+        t0 = torch.cuda.Event(enable_timing=True)
+        t1 = torch.cuda.Event(enable_timing=True)
+        t0.record()
+        for _ in range(iters):
+            fn()
+        t1.record()
+        torch.cuda.synchronize()
+        ts.append(t0.elapsed_time(t1) / iters)
+    return sorted(ts)[len(ts) // 2]
+
+
+def _card():
+    """Device name and power limit, read next to the numbers they qualify."""
+    import torch
+    try:
+        q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()),
+                            "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.TimeoutExpired):
+        q = "nvidia-smi unavailable"
+    return "%s, power limit / max SM clock: %s" % (torch.cuda.get_device_name(), q)
 
 
 def stage(name, arg):
@@ -83,12 +100,17 @@ def stage(name, arg):
             torch.cuda.synchronize()
             out["%dx%dx%d" % (M, K, N)] = _err(dW, a.double().t() @ gy.double())
     elif name == "perf":
+        # the K-major calls of bench.py's DeepFM tower at its batch: forward 624->400 and 400->400
+        # (bias, ReLU, planes, column of ones), dX into masked planes at output widths 400 and
+        # 624, dX into fp32 at 624 (the gradient of the tower input); plus the dW kernel
         M = 65536
+        out["card"] = _card()
         res = {}
+        tm = dict(iters=20, warmup=3, repeats=5)
         for (K, N) in [(624, 400), (400, 400)]:
             x = torch.randn(M, K, device=dev)
             W = torch.randn(K, N, device=dev) / K ** 0.5
-            b = torch.zeros(N, device=dev)
+            b = torch.randn(N, device=dev) * 0.1
             a = ops.raw_tc_split(x)
             Wp, WTp = ops.raw_tc_prep_weight(W)
             gp, _ = ops.raw_tc_split_bwd(torch.randn(M, N, device=dev), None)
@@ -98,18 +120,22 @@ def stage(name, arg):
                 for bk in (64, 32):
                     ops.tc_debug(4, bk)
                     tag = "%dx%d bn%d bk%d" % (K, N, bn, bk)
-                    t = _time(lambda: ops.raw_tc_linear_fwd(a, K, WTp, N, b, True, False, True))
+                    t = _time(lambda: ops.raw_tc_linear_fwd(a, K, WTp, N, b, True, False, True,
+                                                            ones_col=True), **tm)
                     res["fwd " + tag] = [round(t, 4), round(fl / t / 1e9, 1)]
-                    t = _time(lambda: ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, a, False, True, False))
+                    t = _time(lambda: ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, a, False, True, False),
+                              **tm)
                     res["dx  " + tag] = [round(t, 4), round(fl / t / 1e9, 1)]
-                    t = _time(lambda: ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, a, False, True, True))
+                    t = _time(lambda: ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, a, False, True, True),
+                              **tm)
                     res["dx+colsum " + tag] = [round(t, 4), round(fl / t / 1e9, 1)]
-                    t = _time(lambda: ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, None, True, False, False))
+                    t = _time(lambda: ops.raw_tc_linear_bwd_dx(gp, N, Wp, K, None, True, False, False),
+                              **tm)
                     res["dx f32 " + tag] = [round(t, 4), round(fl / t / 1e9, 1)]
-                ops.tc_debug(4, 64)
-                t = _time(lambda: ops.raw_tc_linear_bwd_dw(a, K, gp, N))
+                t = _time(lambda: ops.raw_tc_linear_bwd_dw(a, K, gp, N), **tm)
                 res["dw  %dx%d bn%d" % (K, N, bn)] = [round(t, 4), round(fl / t / 1e9, 1)]
             ops.tc_debug(0, 0)
+            ops.tc_debug(4, 32)
             # library reference: the three bf16 GEMMs of the round-1 path
             a2 = torch.randn(M, 2 * K, device=dev).to(torch.bfloat16)
             w2 = torch.randn(2 * K, N, device=dev).to(torch.bfloat16)
