@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define B200REC_ABI_VERSION 3
+#define B200REC_ABI_VERSION 4
 
 #define B200REC_OK 0
 #define B200REC_ERR_INVALID (-1)   /* bad argument (shape, alignment, NULL) */
@@ -106,6 +106,36 @@ int b200rec_embed_fm_bwd(const float* feat, const float* S, const float* dfeat_d
                          float* ddense_w1, int64_t B, int F, int Dn, int D, void* workspace,
                          size_t workspace_bytes, void* stream);
 
+/* ---- FFM: field-aware second-order term fused with its gather -------------- */
+/* Replaces FFM.forward, models/rank/ffm/net.py:99-133.  NF = F + Dn fields, R = NF*D.
+ * W [V, ldw] holds fused rows [R emb | w1 | pad] (ldw >= R+1, ldw % 4 == 0, base 16-byte aligned).
+ *   e[b,n,:] = W[ids[b,n], 0:R] (n < F; zeros for padding / out-of-range ids)
+ *            = dense[b,n-F] * dense_w[n-F, :]      (n >= F; dense_w [Dn, R])
+ *   y1[b] = sum_f W[ids[b,f], R] + sum_k dense[b,k]*dense_w1[k] (+ bias[0] if bias != NULL)
+ *   y2[b] = sum_{n<m} < e[b,n, m*D:(m+1)*D], e[b,m, n*D:(n+1)*D] >
+ * Nothing of size [B,NF,R] is written.  1 <= F, F+Dn <= 64; one sample's F staged rows plus dense_w
+ * must fit a CTA's shared memory (F=26, Dn=13 fits up to D=32), else B200REC_ERR_INVALID. */
+int b200rec_ffm_fwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                    const float* dense_w, const float* dense_w1, const float* bias, float* y1,
+                    float* y2, int64_t B, int F, int Dn, int D, int64_t V, int64_t padding_idx,
+                    void* stream);
+/* Backward of b200rec_ffm_fwd with gy1 = dL/dy1, gy2 = dL/dy2 [B] and the grouping of the B*F ids
+ * from b200rec_group_ids:
+ *   dW_rows[u, m*D:(m+1)*D] = sum_{(b,f) in segment u, m != f} gy2[b] * e[b,m, f*D:(f+1)*D]
+ *   dW_rows[u, R] = sum gy1[b];  columns R+1 .. ld_dw-1 are written as zeros
+ *   ddense_w[k, m*D:(m+1)*D] = sum_b gy2[b]*dense[b,k]*e[b,m, (F+k)*D:(F+k+1)*D]   (m != F+k)
+ *   ddense_w1[k] = sum_b gy1[b]*dense[b,k];   dbias[0] = sum_b gy1[b] (dbias may be NULL)
+ * Only the first num_unique[0] rows of dW_rows are written, so it needs min(B*F, V) rows.
+ * Ids with more than 64 positions are split over CTAs; every sum has a fixed order, no float
+ * atomics: a second run is bit-identical. */
+int b200rec_ffm_bwd_workspace_bytes(int64_t B, int F, int Dn, int D, size_t* bytes_host);
+int b200rec_ffm_bwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                    const float* dense_w, const float* gy1, const float* gy2,
+                    const int32_t* seg_offsets, const int32_t* sorted_pos,
+                    const int32_t* num_unique, float* dW_rows, int64_t ld_dw, float* ddense_w,
+                    float* ddense_w1, float* dbias, int64_t B, int F, int Dn, int D, int64_t V,
+                    int64_t padding_idx, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- plain gather / segmented scatter-add (W&D, DCN-V2, DIN lookups) ------ */
 /* out[i,:] = W[ids[i],:]  (zeros if ids[i]==padding_idx).  Replaces paddle.nn.Embedding
  * forward (lookup_table_v2), e.g. models/rank/wide_deep/net.py:90, dcn_v2/net.py:95. */
@@ -134,7 +164,8 @@ int b200rec_rows_to_dense(const int64_t* unique_ids, const float* rows, int64_t 
                           int64_t V, void* stream);
 
 /* ---- row-wise ("lazy") optimizers applied to the touched rows only -------- */
-/* W (and m, v) rows start at i*ldw, gradient rows at u*ld_rows; D columns are updated. */
+/* W (and m, v) rows start at i*ldw, gradient rows at u*ld_rows; D columns are updated.  Rows wider
+ * than 128 floats (FFM's [R | w1] rows) are updated by one warp per row in 32-lane chunks. */
 /* W[id] -= lr * g */
 int b200rec_sparse_sgd(float* W, int64_t ldw, const int64_t* unique_ids, const float* rows,
                        int64_t ld_rows, const int32_t* num_unique, int64_t n, int D, int64_t V,

@@ -17,6 +17,7 @@
 #include "hash_keys.cuh"
 #include "dot_interact.cuh"
 #include "din_attn.cuh"
+#include "ffm.cuh"
 
 namespace b200rec {
 
@@ -129,6 +130,45 @@ int b200rec_embed_fm_bwd(const float* feat, const float* S, const float* dfeat_d
                              num_unique, dW_rows, dW1_rows, SegOut{ld_dw, ld_dw1, dw1_zero_pad},
                              ddense_w, ddense_w1, B, F, Dn, D, workspace, workspace_bytes,
                              ST(stream));
+}
+
+int b200rec_ffm_fwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                    const float* dense_w, const float* dense_w1, const float* bias, float* y1,
+                    float* y2, int64_t B, int F, int Dn, int D, int64_t V, int64_t padding_idx,
+                    void* stream) {
+  B200_REQUIRE(B >= 0 && V > 0, "ffm_fwd: bad sizes");
+  if (B > 0) {
+    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(y1); NOT_NULL(y2);
+    if (Dn > 0) { NOT_NULL(dense); NOT_NULL(dense_w); NOT_NULL(dense_w1); }
+  }
+  return launch_ffm_fwd(W, ldw, ids, dense, dense_w, dense_w1, bias, y1, y2, B, F, Dn, D, V,
+                        padding_idx, ST(stream));
+}
+
+int b200rec_ffm_bwd_workspace_bytes(int64_t B, int F, int Dn, int D, size_t* bytes_host) {
+  NOT_NULL(bytes_host);
+  B200_REQUIRE(B >= 0 && F >= 1 && Dn >= 0 && D >= 1 && F + Dn <= kFfmMaxFields,
+               "ffm_bwd_workspace_bytes: bad sizes");
+  *bytes_host = FfmBwdWs(B, F, Dn, D).total;
+  return B200REC_OK;
+}
+
+int b200rec_ffm_bwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                    const float* dense_w, const float* gy1, const float* gy2,
+                    const int32_t* seg_offsets, const int32_t* sorted_pos,
+                    const int32_t* num_unique, float* dW_rows, int64_t ld_dw, float* ddense_w,
+                    float* ddense_w1, float* dbias, int64_t B, int F, int Dn, int D, int64_t V,
+                    int64_t padding_idx, void* workspace, size_t workspace_bytes, void* stream) {
+  B200_REQUIRE(B >= 0 && V > 0, "ffm_bwd: bad sizes");
+  if (Dn > 0) { NOT_NULL(ddense_w); NOT_NULL(ddense_w1); }
+  if (B > 0) {
+    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(gy1); NOT_NULL(gy2); NOT_NULL(seg_offsets);
+    NOT_NULL(sorted_pos); NOT_NULL(num_unique); NOT_NULL(dW_rows); NOT_NULL(workspace);
+    if (Dn > 0) { NOT_NULL(dense); NOT_NULL(dense_w); }
+  }
+  return launch_ffm_bwd(W, ldw, ids, dense, dense_w, gy1, gy2, seg_offsets, sorted_pos,
+                        num_unique, dW_rows, ld_dw, ddense_w, ddense_w1, dbias, B, F, Dn, D, V,
+                        padding_idx, workspace, workspace_bytes, ST(stream));
 }
 
 int b200rec_gather(const float* W, int64_t ldw, const int64_t* ids, float* out, int64_t n, int D,

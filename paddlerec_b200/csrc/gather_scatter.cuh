@@ -291,28 +291,98 @@ row_adagrad_kernel(float* __restrict__ W, float* __restrict__ g2sum,
   }
 }
 
+// Wide rows (more than 32 vector chunks, e.g. FFM's [R emb | w1] rows of 352-1252 floats): one
+// warp per row, each lane stepping through the row 32*VEC floats at a time.
+template <int VEC, typename Op>
+__global__ void __launch_bounds__(kGatherThreads)
+row_update_wide_kernel(const int64_t* __restrict__ unique_ids, const float* __restrict__ rows,
+                       const int32_t* __restrict__ num_unique, int D, int64_t V, int64_t ldw,
+                       int64_t ld_rows, Op op) {
+  constexpr int WPB = kGatherThreads / 32;
+  const int U = num_unique[0];
+  const int r = threadIdx.x % 32;
+  for (int64_t u = (int64_t)blockIdx.x * WPB + threadIdx.x / 32; u < U;
+       u += (int64_t)gridDim.x * WPB) {
+    const int64_t id = unique_ids[u];
+    if ((uint64_t)id >= (uint64_t)V) continue;
+    for (int c = r * VEC; c < D; c += 32 * VEC) {
+      const Vec<VEC> g = ld_row<VEC>(rows + (size_t)u * ld_rows + c);
+      op.template apply<VEC>((size_t)id * ldw + c, g, r);
+    }
+  }
+}
+
+template <int VEC>
+__global__ void __launch_bounds__(kGatherThreads)
+row_adagrad_wide_kernel(float* __restrict__ W, float* __restrict__ g2sum,
+                        const int64_t* __restrict__ unique_ids, const float* __restrict__ rows,
+                        const int32_t* __restrict__ num_unique, int D, int64_t V, int64_t ldw,
+                        int64_t ld_rows, float lr, float g0, float lo, float hi) {
+  constexpr int WPB = kGatherThreads / 32;
+  const int U = num_unique[0];
+  const int r = threadIdx.x % 32;
+  for (int64_t u = (int64_t)blockIdx.x * WPB + threadIdx.x / 32; u < U;
+       u += (int64_t)gridDim.x * WPB) {
+    const int64_t id = unique_ids[u];   // the whole warp holds the same row
+    if ((uint64_t)id >= (uint64_t)V) continue;
+    const float* grow = rows + (size_t)u * ld_rows;
+    const float acc = g2sum[id];
+    float sq = 0.f;
+#pragma unroll 1
+    for (int c = r * VEC; c < D; c += 32 * VEC) {
+      const Vec<VEC> g = ld_row<VEC>(grow + c);
+#pragma unroll
+      for (int k = 0; k < VEC; ++k) sq = fmaf(g.v[k], g.v[k], sq);
+    }
+    sq = group_sum<32>(sq);
+    const float scale = sqrtf(g0 / (g0 + acc));
+#pragma unroll 1
+    for (int c = r * VEC; c < D; c += 32 * VEC) {
+      const Vec<VEC> g = ld_row<VEC>(grow + c);
+      Vec<VEC> w = *reinterpret_cast<const Vec<VEC>*>(W + (size_t)id * ldw + c);
+#pragma unroll
+      for (int k = 0; k < VEC; ++k) {
+        w.v[k] -= lr * g.v[k] * scale;
+        w.v[k] = fminf(fmaxf(w.v[k], lo), hi);
+      }
+      st_plain<VEC>(W + (size_t)id * ldw + c, w);
+    }
+    __syncwarp();
+    if (r == 0) g2sum[id] += sq / (float)D;
+  }
+}
+
 // Row geometry for the row-wise optimizers: start from the widest vector D allows and narrow it
 // until the row strides and base addresses fit (column VIEWS of a table — e.g. the embedding part
-// of a [show, click, emb] GPUBox row — start at a 4- or 8-byte offset).
+// of a [show, click, emb] GPUBox row — start at a 4- or 8-byte offset).  Rows of more than 32
+// chunks get tpr = 0: the wide kernels above.
 static bool pick_row_shape_for(int D, int64_t ldw, int64_t ld_rows, const void* const* ptrs, int np,
                                RowShape* rs) {
-  if (!pick_row_shape(D, rs)) return false;
+  if (D < 1) return false;
   auto fits = [&](int vec) {
     if (D % vec || ldw % vec || ld_rows % vec) return false;
     for (int i = 0; i < np; ++i)
       if (ptrs[i] != nullptr && reinterpret_cast<uintptr_t>(ptrs[i]) % (vec * 4) != 0) return false;
     return true;
   };
-  int vec = rs->vec;
+  int vec = (D % 4 == 0) ? 4 : (D % 2 == 0 ? 2 : 1);
   while (vec > 1 && !fits(vec)) vec >>= 1;
   const int chunks = D / vec;
-  if (chunks > 32) return false;
   int tpr = 1;
   while (tpr < chunks) tpr <<= 1;
   rs->vec = vec;
-  rs->tpr = tpr;
+  rs->tpr = chunks > 32 ? 0 : tpr;
   return true;
 }
+
+#define B200_DISPATCH_VEC(vec, ...)                                   \
+  do {                                                                \
+    switch (vec) {                                                    \
+      case 4: { constexpr int VEC = 4; __VA_ARGS__; } break;          \
+      case 2: { constexpr int VEC = 2; __VA_ARGS__; } break;          \
+      default: { constexpr int VEC = 1; __VA_ARGS__; } break;         \
+    }                                                                 \
+  } while (0)
 
 template <typename Op>
 static int launch_row_update(const char* what, const int64_t* unique_ids, const float* rows,
@@ -324,6 +394,14 @@ static int launch_row_update(const char* what, const int64_t* unique_ids, const 
   B200_REQUIRE(ldw >= D && ld_rows >= D, "%s: bad row strides", what);
   B200_REQUIRE(pick_row_shape_for(D, ldw, ld_rows, ptrs, 4, &rs), "%s: unsupported D=%d", what, D);
   if (n == 0) return B200REC_OK;
+  if (rs.tpr == 0) {
+    constexpr int WPB = kGatherThreads / 32;
+    const unsigned grid = (unsigned)min((n + WPB - 1) / WPB, (int64_t)sm_count() * 64);
+    B200_DISPATCH_VEC(rs.vec, row_update_wide_kernel<VEC, Op><<<grid, kGatherThreads, 0, st>>>(
+                                  unique_ids, rows, num_unique, D, V, ldw, ld_rows, op));
+    B200_LAUNCH_CHECK();
+    return B200REC_OK;
+  }
   B200_DISPATCH_ROW_SHAPE(rs, {
     constexpr int GPB = kGatherThreads / TPR;
     const int64_t want = (n + GPB - 1) / GPB;
@@ -345,6 +423,15 @@ static int launch_adagrad(float* W, float* g2sum, const int64_t* unique_ids, con
   B200_REQUIRE(pick_row_shape_for(D, ldw, ld_rows, ptrs, 2, &rs), "sparse_adagrad: unsupported D=%d",
                D);
   if (n == 0) return B200REC_OK;
+  if (rs.tpr == 0) {
+    constexpr int WPB = kGatherThreads / 32;
+    const unsigned grid = (unsigned)min((n + WPB - 1) / WPB, (int64_t)sm_count() * 64);
+    B200_DISPATCH_VEC(rs.vec, row_adagrad_wide_kernel<VEC><<<grid, kGatherThreads, 0, st>>>(
+                                  W, g2sum, unique_ids, rows, num_unique, D, V, ldw, ld_rows, lr,
+                                  g0, lo, hi));
+    B200_LAUNCH_CHECK();
+    return B200REC_OK;
+  }
   B200_DISPATCH_ROW_SHAPE(rs, {
     constexpr int GPB = kGatherThreads / TPR;
     const int64_t want = (n + GPB - 1) / GPB;

@@ -41,7 +41,7 @@ def _req(t: torch.Tensor, dtype, name: str) -> torch.Tensor:
 # it as `gpu_launches`.  KERNELS_PER_CALL is the static number of our kernels each entry point runs.
 LAUNCHES = 0
 KERNELS_PER_CALL = {
-    "embed_fm_fwd": 1, "group_ids": 3, "embed_fm_bwd": 5, "gather": 1, "segment_reduce": 3,
+    "embed_fm_fwd": 1, "group_ids": 3, "embed_fm_bwd": 5, "ffm_fwd": 1, "ffm_bwd": 5, "gather": 1, "segment_reduce": 3,
     "shard_gather_push": 1, "shard_push_rows": 1, "shard_fm_grads_push": 1, "rows_to_dense": 1, "sparse_sgd": 1, "sparse_adam": 1, "sparse_adagrad": 1, "cross_v2_fwd": 1,
     "cross_v2_bwd": 2, "shard_bucketize": 2, "tower_split": 1, "tower_relu_bwd_split": 2,
     "tower_prep_weight": 1, "tower_fold_dw": 1, "tc_split": 1, "tc_split_bwd": 2,
@@ -273,6 +273,63 @@ def raw_embed_fm_bwd(feat, S, dfeat_dnn, gy1, gy2, dense, seg_offsets, sorted_po
           "embed_fm_bwd")
     _count("embed_fm_bwd")
     return dW_rows, dW1_rows, ddense_w, ddense_w1
+
+
+def raw_ffm_fwd(W, ids, dense, dense_w, dense_w1, bias, padding_idx: int, D: int):
+    """FFM's first- and field-aware second-order terms (b200rec_ffm_fwd).  W: [V, ldw] fused rows
+    [R emb | w1 | pad] with R = (F + Dn) * D; dense_w [Dn, R]; bias [1] or None (added to y1).
+    Returns (y1 [B], y2 [B])."""
+    lib = _lib.load()
+    W = _req(W, torch.float32, "W")
+    ids = _req(ids, torch.int64, "ids")
+    dense = _req(dense, torch.float32, "dense")
+    dense_w = _req(dense_w, torch.float32, "dense_w")
+    dense_w1 = _req(dense_w1, torch.float32, "dense_w1")
+    if bias is not None:
+        bias = _req(bias, torch.float32, "bias")
+    B, F = ids.shape
+    Dn = dense.shape[1]
+    V, ldw = W.shape
+    assert dense.shape[0] == B and dense_w.numel() == Dn * (F + Dn) * D and dense_w1.numel() == Dn
+    y1 = torch.empty(B, dtype=torch.float32, device=W.device)
+    y2 = torch.empty(B, dtype=torch.float32, device=W.device)
+    check(lib.b200rec_ffm_fwd(ptr(W), ldw, ptr(ids), ptr(dense), ptr(dense_w), ptr(dense_w1),
+                              ptr(bias), ptr(y1), ptr(y2), B, F, Dn, D, V, int(padding_idx),
+                              _stream()), "ffm_fwd")
+    _count("ffm_fwd")
+    return y1, y2
+
+
+def raw_ffm_bwd(W, ids, dense, dense_w, gy1, gy2, groups: "IdGroups", padding_idx: int, D: int):
+    """Backward of raw_ffm_fwd.  Returns (dW_rows [min(B*F, V), G] = [R emb | g1 | zeros] with
+    G = fused_grad_cols(R), only the first groups.num[0] rows valid; ddense_w [Dn, R];
+    ddense_w1 [Dn]; dbias [1])."""
+    lib = _lib.load()
+    W = _req(W, torch.float32, "W")
+    ids = _req(ids, torch.int64, "ids")
+    dense = _req(dense, torch.float32, "dense")
+    dense_w = _req(dense_w, torch.float32, "dense_w")
+    gy1 = _req(gy1, torch.float32, "gy1").reshape(-1)
+    gy2 = _req(gy2, torch.float32, "gy2").reshape(-1)
+    B, F = ids.shape
+    Dn = dense.shape[1]
+    V, ldw = W.shape
+    R = (F + Dn) * D
+    G = fused_grad_cols(R)
+    dev = W.device
+    nbytes = ctypes.c_size_t(0)
+    check(lib.b200rec_ffm_bwd_workspace_bytes(B, F, Dn, D, ctypes.byref(nbytes)), "ffm_bwd_ws")
+    ws = workspace(nbytes.value, dev, "ffm_bwd")
+    dW_rows = torch.empty(max(min(B * F, V), 1), G, dtype=torch.float32, device=dev)
+    ddense_w = torch.empty(Dn, R, dtype=torch.float32, device=dev)
+    ddense_w1 = torch.empty(Dn, dtype=torch.float32, device=dev)
+    dbias = torch.empty(1, dtype=torch.float32, device=dev)
+    check(lib.b200rec_ffm_bwd(ptr(W), ldw, ptr(ids), ptr(dense), ptr(dense_w), ptr(gy1), ptr(gy2),
+                              ptr(groups.seg_offsets), ptr(groups.sorted_pos), ptr(groups.num),
+                              ptr(dW_rows), G, ptr(ddense_w), ptr(ddense_w1), ptr(dbias), B, F, Dn,
+                              D, V, int(padding_idx), ptr(ws), ws.numel(), _stream()), "ffm_bwd")
+    _count("ffm_bwd")
+    return dW_rows, ddense_w, ddense_w1, dbias
 
 
 def raw_gather(W: torch.Tensor, ids: torch.Tensor, padding_idx: int,
@@ -862,6 +919,47 @@ class _EmbedFM(torch.autograd.Function):
                 None)
 
 
+class _FFM(torch.autograd.Function):
+    """FFM.forward of models/rank/ffm/net.py:99-133 (plus the bias of FFMLayer, net.py:44, when
+    given) as one kernel each way.  The table gradient goes to `sink.accept_fused` as one
+    SelectedRows of fused rows [R emb | g1 | pad]."""
+
+    @staticmethod
+    def forward(ctx, W, ids, dense, dense_w, dense_w1, bias, padding_idx, sink, D):
+        Dn = dense.shape[1]
+        R = (ids.shape[1] + Dn) * D
+        y1, y2 = raw_ffm_fwd(W, ids, dense, dense_w.reshape(Dn, R), dense_w1.reshape(-1), bias,
+                             padding_idx, D)
+        ctx.save_for_backward(ids, dense, dense_w)
+        ctx.W, ctx.sink, ctx.padding_idx, ctx.D = W, sink, padding_idx, D
+        ctx.dense_w1_shape = dense_w1.shape
+        ctx.bias_shape = None if bias is None else bias.shape
+        return y1.unsqueeze(1), y2.unsqueeze(1)
+
+    @staticmethod
+    def backward(ctx, dy1, dy2):
+        ids, dense, dense_w = ctx.saved_tensors
+        B, Dn = dense.shape
+        dev = dense.device
+        gy1 = dy1.reshape(-1).contiguous() if dy1 is not None else torch.zeros(B, device=dev)
+        gy2 = dy2.reshape(-1).contiguous() if dy2 is not None else torch.zeros(B, device=dev)
+        V = ctx.W.shape[0]
+        groups = ctx.sink.groups_for(ids, V, ctx.padding_idx)
+        R = (ids.shape[1] + Dn) * ctx.D
+        dW_rows, ddense_w, ddense_w1, dbias = raw_ffm_bwd(ctx.W, ids, dense, dense_w.reshape(Dn, R),
+                                                          gy1, gy2, groups, ctx.padding_idx, ctx.D)
+        ctx.sink.accept_fused(SelectedRows(groups.unique_ids, dW_rows, groups.num, V))
+        db = None if ctx.bias_shape is None else dbias.reshape(ctx.bias_shape)
+        return (None, None, None, ddense_w.reshape(dense_w.shape),
+                ddense_w1.reshape(ctx.dense_w1_shape), db, None, None, None)
+
+
+def ffm(W, ids, dense, dense_w, dense_w1, bias, padding_idx, sink, D):
+    """-> (y1 [B,1], y2 [B,1]) of FFM over the fused table W [V, >= R+1]; bias (may be None) is
+    added to y1 and receives its gradient."""
+    return _FFM.apply(W, ids, dense, dense_w, dense_w1, bias, padding_idx, sink, D)
+
+
 def fused_grad_cols(D: int) -> int:
     """Columns of a fused gradient row [D | g1 | pad]: D+1 rounded up to a multiple of 4."""
     return (D + 1 + 3) // 4 * 4
@@ -1407,7 +1505,7 @@ def _wrap_timed(fn, name):
     return timed
 
 
-for _n in ("group_ids", "embed_fm_bwd", "gather", "gather_pool_sum", "segment_reduce", "sparse_sgd",
+for _n in ("group_ids", "embed_fm_bwd", "ffm_fwd", "ffm_bwd", "gather", "gather_pool_sum", "segment_reduce", "sparse_sgd",
            "sparse_adam", "sparse_adagrad", "cross_v2_fwd", "cross_v2_bwd", "shard_bucketize",
            "shard_gather_push", "shard_push_rows", "shard_fm_grads_push",
            "tc_split", "tc_split_bwd", "tc_prep_weight", "tc_linear_fwd", "tc_cross_fwd",
