@@ -401,7 +401,7 @@ def merge_selected_rows(a: SelectedRows, b: SelectedRows) -> SelectedRows:
 def raw_rows_to_dense(sr: SelectedRows, dW: torch.Tensor) -> None:
     lib = _lib.load()
     dW = _req(dW, torch.float32, "dW")
-    n, ld_rows = sr.value.shape
+    n, ld_rows = sr.value.shape[0], sr.value.stride(0)     # column views of a table are allowed
     check(lib.b200rec_rows_to_dense(ptr(sr.rows), ptr(sr.value), ld_rows, ptr(sr.num), ptr(dW),
                                     dW.shape[1], n, sr.cols, sr.height, _stream()), "rows_to_dense")
     _count("rows_to_dense")

@@ -53,6 +53,16 @@ TOWER_ROW_SLICES = 528    # tower.cuh:337 kTowerRowSlices; TX/TY tower.cuh:382-3
 TOWER_THREADS = 256       # tower.cuh:21
 TOWER_UNROLL = 4          # tower.cuh:103 kBwdUnroll
 STREAM_CTAS_PER_SM = 16   # b200rec.cu:577,589,642 (cvm, hash_keys: 256-thread CTAs)
+FFM_THREADS = 256         # ffm.cuh:19  kFfmThreads
+FFM_MAX_FIELDS = 64       # ffm.cuh:20  kFfmMaxFields
+FFM_FWD_MAX_CTAS_PER_SM = 2048 // FFM_THREADS  # ffm.cuh:176-179 grid = min(B, SM*per_sm), per_sm from
+#                           the occupancy call: at most 2048 threads per SM
+FFM_HOT_CHUNK = 1024      # ffm.cuh:228 kFfmHotChunk; items pack c | (chunks << 16) :270
+FFM_MAX_CHUNKS = 32767    # ffm.cuh:406 B*F < 32767 * kFfmHotChunk
+FFM_MAX_SLICES = 256      # ffm.cuh:241 slices = min(256, ceil(B/256))
+FFM_LIGHT_CTAS_PER_SM = 16  # ffm.cuh:431 light grid min(ceil(n/8), 16*SM)
+FFM_HOT_CTAS_PER_SM = 8   # ffm.cuh:436 hot / combine grid min(max_items, 8*SM)
+WIDE_CTAS_PER_SM = 64     # gather_scatter.cuh:399, 428 wide-row grids min(ceil(n/8), 64*SM)
 
 
 def _ops():
@@ -885,3 +895,470 @@ def test_cvm_at_scale(use_cvm):
     assert_loops("cvm_bwd_kernel: elements per thread", N * (D + 2) // (STREAM_CTAS_PER_SM * _sm() * 256))
     dx = ops.raw_cvm_bwd(dy, sc, D, use_cvm)
     assert torch.equal(dx[:, :2], sc) and torch.equal(dx[:, 2:], dy[:, -D:])
+
+
+# ================================================================================================
+# 11. FFM (ffm.cuh): persistent forward, light / hot / combine backward, dense-gradient slices
+# ================================================================================================
+def ffm_staged_cols(R):
+    """ffm_staged_cols, ffm.cuh:22: [R | w1 | pad] rounded up to 4 floats."""
+    return (R + 1 + 3) // 4 * 4
+
+
+def ffm_fwd_smem(F, Dn, D, nbuf):
+    """FfmFwdSmem(F, Dn, D, nbuf).total, ffm.cuh:26-36."""
+    NF = F + Dn
+    R, P = NF * D, NF * (NF - 1) // 2
+    a16 = lambda x: (x + 15) // 16 * 16  # noqa: E731
+    off_pairs = a16(Dn * R * 4)
+    off_red = a16(off_pairs + P * 4)
+    off_buf = off_red + 16 * (FFM_THREADS // 32 + 4)
+    return off_buf + nbuf * F * ffm_staged_cols(R) * 4
+
+
+def _ffm_feat(W, ids, dense, dense_w, s, e, D, pad):
+    """Samples s:e in fp64: e[b, n, :] [b, NF, R] (table rows, zero for padding and out-of-range
+    ids; dense rows x * dense_w), the first-order table terms [b, F] and x [b, Dn]."""
+    V = W.shape[0]
+    F, Dn = ids.shape[1], dense.shape[1]
+    R = (F + Dn) * D
+    idb = ids[s:e]
+    ok = ((idb >= 0) & (idb < V) & (idb != pad)).unsqueeze(2)
+    rows = W[idb.clamp(0, V - 1), :R + 1].double() * ok
+    x = dense[s:e].double()
+    feat = torch.cat([rows[:, :, :R], x.unsqueeze(2) * dense_w.double().unsqueeze(0)], 1)
+    return feat, rows[:, :, R], x
+
+
+def _ffm_table(V, R, g):
+    """Fused rows [R emb | w1 | 123...]: the slot's padding must never be read."""
+    ops = _ops()
+    W = torch.full((V, ops.fused_slot(R)), 123.0, device=DEV)
+    W[:, :R + 1] = torch.randn(V, R + 1, generator=g, device=DEV) * 0.1
+    return W
+
+
+@pytest.mark.parametrize("F,Dn,D,B,nbuf", [
+    (26, 13, 22, None, 2),     # the largest double-buffered shape at F=26, Dn=13
+    (26, 13, 23, None, 1),     # the smallest single-buffered one
+    (26, 13, 16, 65536, 2),
+    (26, 0, 9, None, 2),       # no dense fields
+    (40, 24, 1, None, 2),      # F+Dn = 64 fields: P = 2016 pairs, 8 per thread
+    (26, 13, 1, None, 2),
+])
+def test_ffm_fwd_at_scale(F, Dn, D, B, nbuf):
+    """ffm_fwd_kernel: persistent CTAs, grid = min(B, SM*per_sm) with per_sm <= 2048/256 = 8
+    (ffm.cuh:176-179), so B >= 3*8*SM + 17 makes every CTA take >= 3 samples: with two buffers
+    every CTA stages into both and prefetches across iterations.  The buffering the case gets is
+    asserted from the FfmFwdSmem mirror against the device's opt-in shared-memory limit.
+    y2: each pair is a D-fma dot (D roundings), scaled by sa*sc (1) and fma'd into the thread's
+    accumulator of ceil(P/256) pairs, then 5 shuffle levels and 8 warp partials in order:
+    k = D + ceil(P/256) + 15 of sum over pairs of |e[n, block m]| . |e[m, block n]|.
+    y1: F adds of w1, Dn fmas of x*dense_w1, one add of the two and one of the bias: k = F + Dn + 2.
+    Padding, negative and >= V ids stage zero rows; raw_oob_count counts each out-of-range
+    position exactly once; a second run is bit-identical."""
+    ops = _ops()
+    SM = _sm()
+    NF = F + Dn
+    R, P = NF * D, NF * (NF - 1) // 2
+    assert NF <= FFM_MAX_FIELDS
+    limit = torch.cuda.get_device_properties(0).shared_memory_per_block_optin
+    if nbuf == 2:
+        assert ffm_fwd_smem(F, Dn, D, 2) <= limit, "F=%d Dn=%d D=%d no longer double-buffered" % (F, Dn, D)
+    else:
+        assert ffm_fwd_smem(F, Dn, D, 2) > limit >= ffm_fwd_smem(F, Dn, D, 1), \
+            "F=%d Dn=%d D=%d is no longer the single-buffered case" % (F, Dn, D)
+    B = B or 3 * FFM_FWD_MAX_CTAS_PER_SM * SM + 17
+    assert_loops("ffm_fwd_kernel F=%d Dn=%d D=%d (%d buffers): samples per CTA" % (F, Dn, D, nbuf),
+                 B // (FFM_FWD_MAX_CTAS_PER_SM * SM))
+    V, pad = 20_000, 0
+    g = torch.Generator(device=DEV).manual_seed(1000 * D + NF)
+    W = _ffm_table(V, R, g)
+    ids = torch.randint(1, V, (B, F), generator=g, device=DEV)
+    r = torch.rand(B, F, generator=g, device=DEV)
+    ids[r < 0.03] = pad
+    ids[(r >= 0.03) & (r < 0.035)] = -1 - torch.randint(0, 5, (B, F), generator=g, device=DEV)[
+        (r >= 0.03) & (r < 0.035)]
+    ids[(r >= 0.035) & (r < 0.04)] = V + torch.randint(0, 5, (B, F), generator=g, device=DEV)[
+        (r >= 0.035) & (r < 0.04)]
+    n_oob = int(((ids < 0) | (ids >= V)).sum())
+    assert n_oob > 0 and int((ids == pad).sum()) > 0
+    dense = torch.rand(B, Dn, generator=g, device=DEV)
+    dense_w = torch.randn(Dn, R, generator=g, device=DEV) * 0.1
+    dense_w1 = torch.randn(Dn, generator=g, device=DEV) * 0.1
+    bias = torch.tensor([0.3], device=DEV)
+
+    ops.raw_oob_count()
+    y1, y2 = ops.raw_ffm_fwd(W, ids, dense, dense_w, dense_w1, bias, pad, D)
+    assert ops.raw_oob_count() == n_oob
+
+    f64 = dict(dtype=torch.float64, device=DEV)
+    w1, m1, w2, m2 = (torch.empty(B, **f64) for _ in range(4))
+    iu = torch.triu_indices(NF, NF, 1, device=DEV)
+    chunk = max(1, (1 << 24) // (NF * R))
+    for s in range(0, B, chunk):
+        e = min(B, s + chunk)
+        feat, first, x = _ffm_feat(W, ids, dense, dense_w, s, e, D, pad)
+        e4 = feat.view(e - s, NF, NF, D)
+        prod = e4[:, iu[0], iu[1]] * e4[:, iu[1], iu[0]]
+        w2[s:e], m2[s:e] = prod.sum((1, 2)), prod.abs().sum((1, 2))
+        t1 = torch.cat([first, x * dense_w1.double()], 1)
+        w1[s:e], m1[s:e] = t1.sum(1) + float(bias), t1.abs().sum(1) + abs(float(bias))
+    del feat, e4, prod
+    what = "ffm fwd F=%d Dn=%d D=%d B=%d" % (F, Dn, D, B)
+    assert_within(y2, w2, (D + _cdiv(P, FFM_THREADS) + 15) * U * m2 + 1e-30, what + " y2")
+    assert_within(y1, w1, (F + Dn + 2) * U * m1 + 1e-30, what + " y1")
+    y1b, y2b = ops.raw_ffm_fwd(W, ids, dense, dense_w, dense_w1, bias, pad, D)
+    assert ops.raw_oob_count() == n_oob
+    assert torch.equal(y1, y1b) and torch.equal(y2, y2b), what + ": not bit-reproducible"
+
+
+FFM_BWD_LENS = [64, 65, 1024, 1025, 2048, 2049, 150001]   # ids 1..7; 150001 = 147 hot chunks
+FFM_LIGHT_LO = 10_000                                     # light traffic uses ids FFM_LIGHT_LO..V-1
+
+
+def _ffm_bwd_ids(B, F, V, g):
+    """[B, F] ids: ids 1..7 with exactly FFM_BWD_LENS positions; 3*8*SM + 50 ids (100, 101, ...)
+    of 65-300 positions each; 5000 padding positions (id 0, so padding sits inside the hot runs);
+    40 positions each of V+3 and -2; the rest uniform over [FFM_LIGHT_LO, V), all shuffled."""
+    n = B * F
+    n_hot = 3 * FFM_HOT_CTAS_PER_SM * _sm() + 50
+    parts = [torch.full((c,), 1 + i, dtype=torch.int64, device=DEV) for i, c in enumerate(FFM_BWD_LENS)]
+    lens = torch.randint(HOT_THRESHOLD + 1, 301, (n_hot,), generator=g, device=DEV)
+    parts.append(torch.arange(100, 100 + n_hot, device=DEV).repeat_interleave(lens))
+    parts.append(torch.zeros(5000, dtype=torch.int64, device=DEV))
+    parts.append(torch.full((40,), V + 3, dtype=torch.int64, device=DEV))
+    parts.append(torch.full((40,), -2, dtype=torch.int64, device=DEV))
+    used = sum(p.numel() for p in parts)
+    parts.append(torch.randint(FFM_LIGHT_LO, V, (n - used,), generator=g, device=DEV))
+    ids = torch.cat(parts)
+    return ids[torch.randperm(n, generator=g, device=DEV)].reshape(B, F)
+
+
+def ffm_bwd_chain(counts):
+    """Longest fp32 chain of the columns < R of one gradient row, from its segment length
+    (ffm.cuh:249-345); every term g2 * partner is itself up to 2 roundings (a dense partner is
+    x * dense_w).  Light (<= 64 positions): one lane adds the segment in order, len + 2.  Hot, one
+    chunk: each of 8 warps adds ceil(len/8) positions, the 8 warp sums meet in order,
+    ceil(len/8) + 8 + 2.  Several chunks: 1024/8 = 128 per warp, 8 warp sums, then the combine
+    adds the chunk partials in order, 128 + 8 + chunks + 2."""
+    wpb = FFM_THREADS // 32
+    chunks = (counts + FFM_HOT_CHUNK - 1) // FFM_HOT_CHUNK
+    k_one = (counts + wpb - 1) // wpb + wpb + 2
+    k_many = FFM_HOT_CHUNK // wpb + wpb + chunks + 2
+    return torch.where(counts <= HOT_THRESHOLD, counts + 2,
+                       torch.where(chunks == 1, k_one, k_many)).double()
+
+
+@pytest.mark.parametrize("Dn,D,B", [(13, 9, 65536), (13, 16, 65536), (13, 16, 65536 - 100),
+                                    (0, 9, 65536)])
+def test_ffm_bwd_at_scale(Dn, D, B):
+    """raw_ffm_bwd at B*F = 1.7M positions, F=26, V=200k, ids built by _ffm_bwd_ids so that
+    every light warp walks >= 3 distinct ids, every hot CTA takes >= 3 work items, and the combine
+    adds the 147 chunks of the 150001-position id.  Every row of every distinct id is checked
+    element-wise against the per-position contributions g2[b] * e[b, m, block f] (m != f) and
+    g1[b] merged in fp64 with index_add, bound ffm_bwd_chain(len) for columns < R and 2 less for
+    column R (g1 terms are not rounded); columns R+1..G-1 must be exactly 0.
+    Dense gradients (ffm.cuh:349-391): each of the `slices` = min(256, ceil(B/256)) slices sums
+    per_slice samples with fmaf(g2*x, partner, acc) (+2 roundings per term, +1 for a dense partner's
+    x*dense_w), then the slice partials are added in order: ddense_w k = per_slice + 3 + slices,
+    ddense_w1 k = per_slice + 1 + slices, dbias k = per_slice + slices.  B = 65436 leaves the last
+    slice short.  Every output is bit-identical on a second run."""
+    ops = _ops()
+    SM = _sm()
+    F, V, pad = 26, 200_000, 0
+    NF = F + Dn
+    R = NF * D
+    G = ffm_staged_cols(R)
+    n = B * F
+    g = torch.Generator(device=DEV).manual_seed(100 * D + Dn + B)
+    ids = _ffm_bwd_ids(B, F, V, g)
+    flat = ids.reshape(-1)
+    valid = (flat >= 0) & (flat < V) & (flat != pad)
+    uniq, inv, counts = torch.unique(flat[valid], return_inverse=True, return_counts=True)
+    Uq = uniq.numel()
+    # the loop counts the construction gives
+    assert sorted(counts[counts > 300].tolist()) == sorted(c for c in FFM_BWD_LENS if c > 300)
+    wpb = FFM_THREADS // 32
+    n_light = int((counts <= HOT_THRESHOLD).sum())
+    assert n_light >= 3 * FFM_LIGHT_CTAS_PER_SM * SM * wpb
+    lgrid = min(_cdiv(n, wpb), FFM_LIGHT_CTAS_PER_SM * SM)
+    assert_loops("ffm_bwd_light_kernel: distinct ids per warp", Uq // (lgrid * wpb))
+    hot = counts[counts > HOT_THRESHOLD]
+    n_items = int(((hot + FFM_HOT_CHUNK - 1) // FFM_HOT_CHUNK).sum())
+    max_items = n // (HOT_THRESHOLD + 1) + 1
+    hgrid = min(max_items, FFM_HOT_CTAS_PER_SM * SM)
+    assert_loops("ffm_bwd_hot_kernel: work items per CTA", n_items // hgrid)
+    assert_loops("ffm_bwd_combine_kernel: chunks of the 150001-position id",
+                 _cdiv(FFM_BWD_LENS[-1], FFM_HOT_CHUNK))
+    slices = min(FFM_MAX_SLICES, _cdiv(B, 256))
+    per_slice = _cdiv(B, slices)
+    assert_loops("ffm_bwd_dense_kernel: samples per slice", per_slice)
+
+    W = _ffm_table(V, R, g)
+    dense = torch.rand(B, Dn, generator=g, device=DEV)
+    dense_w = torch.randn(Dn, R, generator=g, device=DEV) * 0.1
+    gy1 = torch.randn(B, generator=g, device=DEV)
+    gy2 = torch.randn(B, generator=g, device=DEV)
+    groups = ops.raw_group_ids(ids, V, pad)
+    assert int(groups.num[0]) == Uq
+    assert torch.equal(groups.unique_ids[:Uq], uniq), "the gradient rows must be exactly the valid ids"
+    out = ops.raw_ffm_bwd(W, ids, dense, dense_w, gy1, gy2, groups, pad, D)
+    out2 = ops.raw_ffm_bwd(W, ids, dense, dense_w, gy1, gy2, groups, pad, D)
+    what = "ffm bwd Dn=%d D=%d B=%d" % (Dn, D, B)
+    assert torch.equal(out[0][:Uq], out2[0][:Uq]), what + ": rows not bit-reproducible"
+    for a, b in zip(out[1:], out2[1:]):
+        assert torch.equal(a, b), what + ": dense gradients not bit-reproducible"
+    del out2
+    dW, ddw, ddw1, db = out
+
+    f64 = dict(dtype=torch.float64, device=DEV)
+    pos_row = torch.full((n,), -1, dtype=torch.int64, device=DEV)
+    pos_row[valid] = inv
+    want, mag = torch.zeros(Uq, R + 1, **f64), torch.zeros(Uq, R + 1, **f64)
+    wdw, mdw = torch.zeros(Dn, NF, D, **f64), torch.zeros(Dn, NF, D, **f64)
+    wd1, md1 = torch.zeros(Dn, **f64), torch.zeros(Dn, **f64)
+    ar = torch.arange(NF, device=DEV)
+    off = (ar[:F].unsqueeze(1) != ar).double().reshape(1, F, NF, 1)          # m != f
+    offd = (ar[F:].unsqueeze(1) != ar).double().unsqueeze(2)                  # m != F+k
+    chunk = 1024
+    for s in range(0, B, chunk):
+        e = min(B, s + chunk)
+        b = e - s
+        feat, _, x = _ffm_feat(W, ids, dense, dense_w, s, e, D, pad)
+        e4 = feat.view(b, NF, NF, D)                       # e4[b, m, f] = e[b, m, block f]
+        g2, g1 = gy2[s:e].double(), gy1[s:e].double()
+        t = e4.transpose(1, 2)[:, :F] * off * g2.view(b, 1, 1, 1)
+        t = torch.cat([t.reshape(b * F, R), g1.repeat_interleave(F).unsqueeze(1)], 1)
+        r = pos_row[s * F:e * F]
+        ok = r >= 0
+        want.index_add_(0, r[ok], t[ok])
+        mag.index_add_(0, r[ok], t[ok].abs())
+        del t
+        if Dn:
+            term = e4[:, :, F:] * (g2.unsqueeze(1) * x).view(b, 1, Dn, 1)    # [b, m, k, D]
+            wdw += term.sum(0).transpose(0, 1) * offd
+            mdw += term.abs().sum(0).transpose(0, 1) * offd
+            wd1 += (g1.unsqueeze(1) * x).sum(0)
+            md1 += (g1.abs().unsqueeze(1) * x.abs()).sum(0)
+    del feat, e4
+    k = ffm_bwd_chain(counts).unsqueeze(1)
+    for r0 in range(0, Uq, 32768):
+        sl = slice(r0, min(Uq, r0 + 32768))
+        bound = k[sl] * U * mag[sl]
+        bound[:, R] -= 2 * U * mag[sl, R]
+        assert_within(dW[sl, :R + 1], want[sl], bound + 1e-30, what + " rows %d.." % r0)
+    assert not dW[:Uq, R + 1:G].any(), what + ": the padding columns of the rows must be 0"
+    del want, mag
+    if Dn:
+        assert_within(ddw, wdw.reshape(Dn, R), (per_slice + 3 + slices) * U * mdw.reshape(Dn, R) + 1e-30,
+                      what + " ddense_w")
+        assert_within(ddw1, wd1, (per_slice + 1 + slices) * U * md1 + 1e-30, what + " ddense_w1")
+    assert_within(db, gy1.double().sum().reshape(1),
+                  (per_slice + slices) * U * gy1.double().abs().sum().reshape(1), what + " dbias")
+
+
+def test_ffm_bwd_chunk_packing_limit():
+    """Work items pack chunk | (chunks << 16) into one int32 (ffm.cuh:270), which the launcher
+    bounds by B*F < 32767*1024 (ffm.cuh:406).  At F=1, Dn=0, D=1 and B*F = 32767*1024 - 1, id 1
+    takes 32766*1024 + 512 positions (32767 chunks: chunk index 32766, chunks << 16 =
+    2,147,418,112), all with gy1 = 1.0; the other 511 positions go to distinct ids.  Each full chunk
+    sums to exactly 1024 (8 warps of 128 ones), and every partial total of the combine is an even
+    integer below 2^25, so id 1's g1 column must be exactly 32766*1024 + 512: a dropped or
+    duplicated chunk shows.  The single-position rows hold their gy1 exactly.  dbias:
+    k = per_slice + slices.  One more position, with every buffer sized for it, is refused with
+    B200REC_ERR_INVALID naming B*F."""
+    import ctypes
+    from paddlerec_b200 import _lib
+    ops = _ops()
+    lib = _lib.load()
+    SM = _sm()
+    n_max = FFM_MAX_CHUNKS * FFM_HOT_CHUNK        # the first B*F the launcher refuses
+    n = n_max - 1
+    n_a = (FFM_MAX_CHUNKS - 1) * FFM_HOT_CHUNK + FFM_HOT_CHUNK // 2
+    chunks = _cdiv(n_a, FFM_HOT_CHUNK)
+    assert chunks == FFM_MAX_CHUNKS and chunks - 1 < 1 << 16 and chunks << 16 == 2_147_418_112
+    assert n_a < 1 << 25 and n_a % 2 == 0
+    hgrid = min(n // (HOT_THRESHOLD + 1) + 1, FFM_HOT_CTAS_PER_SM * SM)
+    assert_loops("ffm_bwd_hot_kernel at the packing limit: work items per CTA", chunks // hgrid)
+    V, A = 1024, 1
+    R = 1
+    G = ffm_staged_cols(R)
+    g = torch.Generator(device=DEV).manual_seed(32767)
+    ids = torch.full((n_max, 1), 2, dtype=torch.int64, device=DEV)
+    body = torch.cat([torch.full((n_a,), A, dtype=torch.int64, device=DEV),
+                      torch.arange(2, 2 + n - n_a, device=DEV)])
+    ids[:n, 0] = body[torch.randperm(n, generator=g, device=DEV)]
+    del body
+    gy1 = torch.where(ids[:, 0] == A, 1.0, torch.randn(n_max, generator=g, device=DEV))
+    gy2 = torch.randn(n_max, generator=g, device=DEV)
+    W = _ffm_table(V, R, g)
+    dense = torch.empty(n_max, 0, device=DEV)
+    dense_w = torch.empty(0, R, device=DEV)
+    groups = ops.raw_group_ids(ids[:n], V, -1)
+    Uq = int(groups.num[0])
+    assert Uq == 1 + n - n_a
+    assert torch.equal(groups.unique_ids[:Uq], torch.arange(1, 1 + Uq, device=DEV))
+    dW, _, _, db = ops.raw_ffm_bwd(W, ids[:n], dense[:n], dense_w, gy1[:n], gy2[:n], groups, -1, 1)
+    assert float(dW[0, R]) == float(n_a), "g1 of the 32767-chunk id: %r, want %d" % (float(dW[0, R]), n_a)
+    want1 = torch.zeros(V, device=DEV)
+    rest = ids[:n, 0] != A
+    want1[ids[:n, 0][rest]] = gy1[:n][rest]
+    assert torch.equal(dW[1:Uq, R], want1[2:1 + Uq])
+    assert not dW[:Uq, :R].any() and not dW[:Uq, R + 1:G].any()
+    slices = min(FFM_MAX_SLICES, _cdiv(n, 256))
+    g1 = gy1[:n].double()
+    assert_within(db, g1.sum().reshape(1), (_cdiv(n, slices) + slices) * U * g1.abs().sum().reshape(1),
+                  "dbias at the packing limit")
+
+    nbytes = ctypes.c_size_t(0)
+    assert lib.b200rec_ffm_bwd_workspace_bytes(n_max, 1, 0, R, ctypes.byref(nbytes)) == 0
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=DEV)
+    seg = torch.zeros(n_max + 1, dtype=torch.int32, device=DEV)
+    pos = torch.zeros(n_max, dtype=torch.int32, device=DEV)
+    num = torch.tensor([Uq, n_max], dtype=torch.int32, device=DEV)
+    out = torch.zeros(V, G, device=DEV)
+    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
+    rc = lib.b200rec_ffm_bwd(P(W), W.stride(0), P(ids), None, None, P(gy1), P(gy2), P(seg), P(pos),
+                             P(num), P(out), G, None, None, P(db), n_max, 1, 0, R, V, -1, P(ws),
+                             nbytes.value, None)
+    assert rc == -1 and b"B*F" in lib.b200rec_last_error(), (rc, lib.b200rec_last_error())
+
+
+# ================================================================================================
+# 12. Wide-row optimizers (gather_scatter.cuh:294-353): one warp per row of > 32 vector chunks
+# ================================================================================================
+ROW_GUARD = 4   # rows of every table / state buffer before and after the V rows the call sees
+
+
+def row_shape_for(D, ldw, ld_rows, byte_offsets):
+    """pick_row_shape_for, gather_scatter.cuh:359-376: (VEC, TPR), TPR = 0 for the wide kernels."""
+    vec = 4 if D % 4 == 0 else (2 if D % 2 == 0 else 1)
+    while vec > 1 and (D % vec or ldw % vec or ld_rows % vec or any(o % (4 * vec) for o in byte_offsets)):
+        vec >>= 1
+    chunks = D // vec
+    tpr = 1
+    while tpr < chunks:
+        tpr <<= 1
+    return vec, (0 if chunks > 32 else tpr)
+
+
+# name: (columns updated, table row stride, gradient row stride, first column of the view, VEC, TPR)
+WIDE_CASES = {
+    "ffm_d9": (352, 384, 352, 0, 4, 0),     # FFM's G at D=9, ldw = fused_slot(R)
+    "ffm_d16": (628, 640, 628, 0, 4, 0),    # FFM's G at D=16
+    "vec1": (625, 640, 625, 0, 1, 0),
+    "cvm_view": (624, 628, 626, 2, 2, 0),   # [show, click, emb] rows: columns 2.. of table and grad
+    "cvm_view_narrow": (16, 20, 18, 2, 2, 8),   # the same view on the lane-group kernels
+}
+
+
+@pytest.mark.parametrize("case", list(WIDE_CASES))
+def test_wide_row_optimizers_at_scale(case):
+    """row_update_wide_kernel (SGD, lazy Adam, rows_to_dense) and row_adagrad_wide_kernel: grid =
+    min(ceil(n/8), 64*SM) warps of one row each (gather_scatter.cuh:399, 428), so U >= 3*8*64*SM
+    rows make every warp update >= 3 rows; each lane steps through the row 32*VEC floats at a
+    time.  Widths: FFM's G at D=9 and D=16 with ldw = fused_slot(R) and separate [V, slot] moments
+    (optim.Adam on FFMLayer), 625 (VEC 1), and a [show, click, emb] column view 2 floats into the
+    table and the gradient (VEC narrowed to 2; optim._table_parts), also at 16 columns on the
+    lane-group kernels (row_update_kernel / row_adagrad_kernel, >= 3 rows per group).
+    Bounds as test_row_updates_at_scale, except AdaGrad's g2sum on the wide kernel: each lane fmas
+    ceil(D/(32*VEC))*VEC squares, 5 shuffle levels, the division by D and the add:
+    k = ceil(D/(32*VEC))*VEC + 5 + 2 per step.  Out-of-range ids among the unique rows (-3, -1, V,
+    V+2) are skipped; untouched rows, moments, g2sum, the guard rows around the V rows and the
+    columns outside the view are bit-identical."""
+    ops = _ops()
+    SM = _sm()
+    Dw, ldw, ldr, c0, vec, tpr = WIDE_CASES[case]
+    assert row_shape_for(Dw, ldw, ldr, [4 * c0, 4 * ROW_GUARD * ldw]) == (vec, tpr)
+    assert row_shape_for(Dw, Dw, ldr, [4 * c0, 4 * ROW_GUARD * Dw]) == (vec, tpr)   # rows_to_dense
+    gpb = ROW_THREADS // (tpr or 32)
+    Uq = 3 * WIDE_CTAS_PER_SM * SM * gpb + 77
+    V = Uq + Uq // 8
+    oob = torch.tensor([-3, -1, V, V + 2], device=DEV)
+    n = Uq + oob.numel()
+    grid = min(_cdiv(n, gpb), WIDE_CTAS_PER_SM * SM)
+    assert_loops("%s (%s): rows per %s" % ("row_update_kernel" if tpr else "row_update_wide_kernel",
+                                           case, "lane group" if tpr else "warp"), n // (grid * gpb))
+    g = torch.Generator(device=DEV).manual_seed(Dw + c0)
+    rows = torch.cat([torch.randperm(V, generator=g, device=DEV)[:Uq].sort().values, oob])
+    rows = rows[torch.randperm(n, generator=g, device=DEV)]
+    ok = (rows >= 0) & (rows < V)
+    val_full = torch.randn(n, ldr, generator=g, device=DEV)
+    num = torch.tensor([n, n], dtype=torch.int32, device=DEV)
+    sr = ops.SelectedRows(rows, val_full[:, c0:], num, V, ncols=Dw)
+    ids = rows[ok]
+    gv = val_full[ok, c0:c0 + Dw]
+    cols = slice(c0, c0 + Dw)
+    inner = slice(ROW_GUARD, ROW_GUARD + V)
+    W0_full = torch.randn(V + 2 * ROW_GUARD, ldw, generator=g, device=DEV)
+    W0 = W0_full[inner, cols]
+    ch = 32768
+
+    def outside_unchanged(full, full0, c=cols):
+        chk = full.clone()
+        if full.dim() == 2:
+            chk[ROW_GUARD + ids, c] = full0[ROW_GUARD + ids, c]
+        else:
+            chk[ROW_GUARD + ids] = full0[ROW_GUARD + ids]
+        return torch.equal(chk, full0)
+
+    # rows_to_dense: zeros + g, exact copies
+    dW_full = torch.zeros(V + 2 * ROW_GUARD, Dw, device=DEV)
+    ops.raw_rows_to_dense(sr, dW_full[inner])
+    assert torch.equal(dW_full[ROW_GUARD + ids], gv), "rows_to_dense " + case
+    assert outside_unchanged(dW_full, torch.zeros_like(dW_full), slice(None)), "rows_to_dense " + case
+    del dW_full
+
+    W_full = W0_full.clone()
+    ops.raw_sparse_sgd(W_full[inner, cols], sr, 0.1)
+    for s in range(0, ids.numel(), ch):
+        i, gg = ids[s:s + ch], gv[s:s + ch].double()
+        want = W0[i].double() - 0.1 * gg
+        assert_within(W_full[inner, cols][i], want, 2 * U * (want.abs() + 0.1 * gg.abs()), "sgd " + case)
+    assert outside_unchanged(W_full, W0_full), "sgd " + case
+
+    W_full = W0_full.clone()
+    m_full, v_full = torch.zeros_like(W0_full), torch.zeros_like(W0_full)
+    b1, b2, eps, lr = 0.9, 0.999, 1e-8, 1e-3
+    for t in (1, 2):
+        ops.raw_sparse_adam(W_full[inner, cols], m_full[inner, cols], v_full[inner, cols], sr, lr, b1, b2,
+                            eps, b1 ** t, b2 ** t)
+    for s in range(0, ids.numel(), ch):
+        i, gg = ids[s:s + ch], gv[s:s + ch].double()
+        Wr, mr, vr = W0[i].double(), torch.zeros_like(gg), torch.zeros_like(gg)
+        mm, upd = torch.zeros_like(gg), torch.zeros_like(gg)
+        for t in (1, 2):                      # oracle/optim.py adam_lazy, with its error magnitudes
+            lr_t = lr * math.sqrt(1 - b2 ** t) / (1 - b1 ** t)
+            den = eps * math.sqrt(1 - b2 ** t)
+            mr = b1 * mr + (1 - b1) * gg
+            vr = b2 * vr + (1 - b2) * gg * gg
+            Wr = Wr - lr_t * mr / (vr.sqrt() + den)
+            mm = b1 * mm + (1 - b1) * gg.abs()
+            upd += lr_t * (10 * mm + 16 * mr.abs()) / (vr.sqrt() + den)
+        assert_within(m_full[inner, cols][i], mr, 10 * U * mm, "adam m " + case)
+        assert_within(v_full[inner, cols][i], vr, 12 * U * vr, "adam v " + case)
+        assert_within(W_full[inner, cols][i], Wr, U * (2 * Wr.abs() + upd), "adam W " + case)
+    assert outside_unchanged(W_full, W0_full), "adam W " + case
+    assert outside_unchanged(m_full, torch.zeros_like(m_full)), "adam m " + case
+    assert outside_unchanged(v_full, torch.zeros_like(v_full)), "adam v " + case
+    del m_full, v_full
+
+    W_full = W0_full.clone()
+    g2_full = torch.zeros(V + 2 * ROW_GUARD, device=DEV)
+    lr, g0, lo, hi = 0.05, 3.0, -2.5, 2.5
+    for _ in range(2):
+        ops.raw_sparse_adagrad(W_full[inner, cols], g2_full[inner], sr, lr, g0, lo, hi)
+    k_g2 = (_cdiv(Dw, 32 * vec) * vec + 5 + 2) if tpr == 0 else Dw + 8
+    for s in range(0, ids.numel(), ch):
+        i, gg = ids[s:s + ch], gv[s:s + ch].double()
+        Wr, g2r, upd = W0[i].double(), torch.zeros(i.numel(), dtype=torch.float64, device=DEV), 0
+        for _ in range(2):                    # oracle/optim.py adagrad_row
+            sc = (g0 / (g0 + g2r)).sqrt().unsqueeze(1)
+            upd = upd + (Dw + 16) * lr * gg.abs() * sc
+            Wr = (Wr - lr * gg * sc).clamp(lo, hi)
+            g2r = g2r + (gg * gg).mean(1)
+        assert_within(g2_full[inner][i], g2r, 2 * k_g2 * U * g2r, "adagrad g2sum " + case)
+        assert_within(W_full[inner, cols][i], Wr, U * (2 * Wr.abs() + upd), "adagrad W " + case)
+    assert outside_unchanged(W_full, W0_full), "adagrad W " + case
+    assert outside_unchanged(g2_full, torch.zeros_like(g2_full)), "adagrad g2sum " + case
