@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define B200REC_ABI_VERSION 4
+#define B200REC_ABI_VERSION 5
 
 #define B200REC_OK 0
 #define B200REC_ERR_INVALID (-1)   /* bad argument (shape, alignment, NULL) */
@@ -135,6 +135,49 @@ int b200rec_ffm_bwd(const float* W, int64_t ldw, const int64_t* ids, const float
                     const int32_t* num_unique, float* dW_rows, int64_t ld_dw, float* ddense_w,
                     float* ddense_w1, float* dbias, int64_t B, int F, int Dn, int D, int64_t V,
                     int64_t padding_idx, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- FAT-DeepFFM: CENet field attention + field-aware Hadamard interaction -- */
+/* Replaces CENLayer.forward and DeepFFM.forward, models/rank/fat_deepffm/net.py:105-151, 219-251,
+ * around the attention MLP (which stays a pair of GEMMs).  NF = F + Dn, R = NF*D, P = NF(NF-1)/2.
+ * W [V, ldw] holds FFM's fused rows (ldw >= R+1, ldw % 4 == 0, base 16-byte aligned); its w1
+ * column is not read.  e[b,n,:] = W[ids[b,n], 0:R] (n < F; zeros for padding / out-of-range ids),
+ * dense[b,n-F] * dense_w[n-F, :] (n >= F).  Same shape limits as b200rec_ffm_fwd, and the sample
+ * buffers also hold one [NF*NF] attention row.
+ *   pool[b, n*NF+m] = max_d e[b,n, m*D+d]
+ * Padding and out-of-range ids are counted (b200rec_oob_count) by this call only. */
+int b200rec_fat_ffm_pool_fwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                             const float* dense_w, float* pool, int64_t B, int F, int Dn, int D,
+                             int64_t V, int64_t padding_idx, void* stream);
+/* With attn [B, NF*NF] and s[b,n,m,:] = attn[b, n*NF+m] * e[b,n, m*D:(m+1)*D]:
+ *   y1[b] = sum_{n,m,d} s[b,n,m,d] (+ bias[0] if bias != NULL), summed in a fixed order
+ *   h[b, p(n,m)*D + d] = s[b,n,m,d] * s[b,m,n,d]   for n < m in row-major pair order
+ * Nothing of size [B,NF,R] is written. */
+int b200rec_fat_ffm_fwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                        const float* dense_w, const float* attn, const float* bias, float* y1,
+                        float* h, int64_t B, int F, int Dn, int D, int64_t V, int64_t padding_idx,
+                        void* stream);
+/* dattn[b, n*NF+m] = sum_d e[b,n,m*D+d] * (gy1[b] + [n != m] * dh[b, p(n,m)*D+d] * s[b,m,n,d]) */
+int b200rec_fat_ffm_bwd_attn(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                             const float* dense_w, const float* attn, const float* gy1,
+                             const float* dh, float* dattn, int64_t B, int F, int Dn, int D,
+                             int64_t V, int64_t padding_idx, void* stream);
+/* Table and dense-parameter gradients through both routes (the attention product and the max
+ * pool), with the grouping of the B*F ids from b200rec_group_ids.  For row n, block m, column j:
+ *   de = attn[n,m] * (gy1 + [m != n] * dh[p(n,m), j] * attn[m,n] * e[m, n*D+j])
+ *        + [j = FIRST argmax_d e[n, m*D+d]] * dpool[n*NF+m]
+ *   dW_rows[u, 0:R] = sum over the positions of segment u of de;  columns R .. ld_dw-1 are 0
+ *   ddense_w[k, c] = sum_b dense[b,k] * de(b, F+k, c);   dbias[0] = sum_b gy1[b] (may be NULL)
+ * The argmax of a dense block is taken on the fp32 product dense * dense_w.  Only the first
+ * num_unique[0] rows of dW_rows are written, so it needs min(B*F, V) rows.  Every sum has a fixed
+ * order, no float atomics: a second run is bit-identical. */
+int b200rec_fat_ffm_bwd_workspace_bytes(int64_t B, int F, int Dn, int D, size_t* bytes_host);
+int b200rec_fat_ffm_bwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                        const float* dense_w, const float* attn, const float* gy1, const float* dh,
+                        const float* dpool, const int32_t* seg_offsets, const int32_t* sorted_pos,
+                        const int32_t* num_unique, float* dW_rows, int64_t ld_dw, float* ddense_w,
+                        float* dbias, int64_t B, int F, int Dn, int D, int64_t V,
+                        int64_t padding_idx, void* workspace, size_t workspace_bytes,
+                        void* stream);
 
 /* ---- plain gather / segmented scatter-add (W&D, DCN-V2, DIN lookups) ------ */
 /* out[i,:] = W[ids[i],:]  (zeros if ids[i]==padding_idx).  Replaces paddle.nn.Embedding

@@ -64,7 +64,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     return LIB_PATH
 
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 _P = c_void_p
 _SIG = {
     "b200rec_abi_version": (c_int, []),
@@ -85,6 +85,17 @@ _SIG = {
     "b200rec_ffm_bwd": (c_int, [_P, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, _P, _P,
                                 _P, c_int64, c_int, c_int, c_int, c_int64, c_int64, _P, c_size_t,
                                 _P]),
+    "b200rec_fat_ffm_pool_fwd": (c_int, [_P, c_int64, _P, _P, _P, _P, c_int64, c_int, c_int, c_int,
+                                         c_int64, c_int64, _P]),
+    "b200rec_fat_ffm_fwd": (c_int, [_P, c_int64, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int, c_int,
+                                    c_int, c_int64, c_int64, _P]),
+    "b200rec_fat_ffm_bwd_attn": (c_int, [_P, c_int64, _P, _P, _P, _P, _P, _P, _P, c_int64, c_int,
+                                         c_int, c_int, c_int64, c_int64, _P]),
+    "b200rec_fat_ffm_bwd_workspace_bytes": (c_int, [c_int64, c_int, c_int, c_int,
+                                                    POINTER(c_size_t)]),
+    "b200rec_fat_ffm_bwd": (c_int, [_P, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64,
+                                    _P, _P, c_int64, c_int, c_int, c_int, c_int64, c_int64, _P,
+                                    c_size_t, _P]),
     "b200rec_gather": (c_int, [_P, c_int64, _P, _P, c_int64, c_int, c_int64, c_int64, _P]),
     "b200rec_segment_reduce_workspace_bytes": (c_int, [c_int64, c_int, POINTER(c_size_t)]),
     "b200rec_segment_reduce": (c_int, [_P, _P, _P, _P, _P, _P, c_int64, c_int, _P, c_size_t, _P]),

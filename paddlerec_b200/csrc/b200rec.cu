@@ -18,6 +18,7 @@
 #include "dot_interact.cuh"
 #include "din_attn.cuh"
 #include "ffm.cuh"
+#include "fat_ffm.cuh"
 
 namespace b200rec {
 
@@ -169,6 +170,76 @@ int b200rec_ffm_bwd(const float* W, int64_t ldw, const int64_t* ids, const float
   return launch_ffm_bwd(W, ldw, ids, dense, dense_w, gy1, gy2, seg_offsets, sorted_pos,
                         num_unique, dW_rows, ld_dw, ddense_w, ddense_w1, dbias, B, F, Dn, D, V,
                         padding_idx, workspace, workspace_bytes, ST(stream));
+}
+
+int b200rec_fat_ffm_pool_fwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                             const float* dense_w, float* pool, int64_t B, int F, int Dn, int D,
+                             int64_t V, int64_t padding_idx, void* stream) {
+  B200_REQUIRE(B >= 0 && V > 0, "fat_ffm_pool_fwd: bad sizes");
+  if (B > 0) {
+    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(pool);
+    if (Dn > 0) { NOT_NULL(dense); NOT_NULL(dense_w); }
+  }
+  return launch_fat_ffm_pool(W, ldw, ids, dense, dense_w, pool, B, F, Dn, D, V, padding_idx,
+                             ST(stream));
+}
+
+int b200rec_fat_ffm_fwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                        const float* dense_w, const float* attn, const float* bias, float* y1,
+                        float* h, int64_t B, int F, int Dn, int D, int64_t V, int64_t padding_idx,
+                        void* stream) {
+  B200_REQUIRE(B >= 0 && V > 0, "fat_ffm_fwd: bad sizes");
+  if (B > 0) {
+    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(attn); NOT_NULL(y1); NOT_NULL(h);
+    if (Dn > 0) { NOT_NULL(dense); NOT_NULL(dense_w); }
+  }
+  const FatSampleArgs a{W, ldw, ids, dense, dense_w, attn, bias, nullptr, nullptr, y1, h,
+                        B, F, Dn, D, V, padding_idx};
+  return launch_fat_sample<false>("fat_ffm_fwd", a, ST(stream));
+}
+
+int b200rec_fat_ffm_bwd_attn(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                             const float* dense_w, const float* attn, const float* gy1,
+                             const float* dh, float* dattn, int64_t B, int F, int Dn, int D,
+                             int64_t V, int64_t padding_idx, void* stream) {
+  B200_REQUIRE(B >= 0 && V > 0, "fat_ffm_bwd_attn: bad sizes");
+  if (B > 0) {
+    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(attn); NOT_NULL(gy1); NOT_NULL(dh); NOT_NULL(dattn);
+    if (Dn > 0) { NOT_NULL(dense); NOT_NULL(dense_w); }
+  }
+  const FatSampleArgs a{W, ldw, ids, dense, dense_w, attn, nullptr, gy1, dh, nullptr, dattn,
+                        B, F, Dn, D, V, padding_idx};
+  return launch_fat_sample<true>("fat_ffm_bwd_attn", a, ST(stream));
+}
+
+int b200rec_fat_ffm_bwd_workspace_bytes(int64_t B, int F, int Dn, int D, size_t* bytes_host) {
+  NOT_NULL(bytes_host);
+  B200_REQUIRE(B >= 0 && F >= 1 && Dn >= 0 && D >= 1 && F + Dn <= kFfmMaxFields,
+               "fat_ffm_bwd_workspace_bytes: bad sizes");
+  *bytes_host = FfmBwdWs(B, F, Dn, D).total;
+  return B200REC_OK;
+}
+
+int b200rec_fat_ffm_bwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
+                        const float* dense_w, const float* attn, const float* gy1, const float* dh,
+                        const float* dpool, const int32_t* seg_offsets, const int32_t* sorted_pos,
+                        const int32_t* num_unique, float* dW_rows, int64_t ld_dw, float* ddense_w,
+                        float* dbias, int64_t B, int F, int Dn, int D, int64_t V,
+                        int64_t padding_idx, void* workspace, size_t workspace_bytes,
+                        void* stream) {
+  B200_REQUIRE(B >= 0 && V > 0, "fat_ffm_bwd: bad sizes");
+  if (Dn > 0) NOT_NULL(ddense_w);
+  if (B > 0) {
+    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(attn); NOT_NULL(gy1); NOT_NULL(dh); NOT_NULL(dpool);
+    NOT_NULL(seg_offsets); NOT_NULL(sorted_pos); NOT_NULL(num_unique); NOT_NULL(dW_rows);
+    NOT_NULL(workspace);
+    if (Dn > 0) { NOT_NULL(dense); NOT_NULL(dense_w); }
+  }
+  const int NF = F + Dn, R = NF * D;
+  const FatBwd a{W, ldw, ids, dense, dense_w, gy1, dh, attn, dpool, F, Dn, D, R,
+                 ffm_staged_cols(R), NF, V, padding_idx};
+  return launch_fat_ffm_bwd(a, seg_offsets, sorted_pos, num_unique, dW_rows, ld_dw, ddense_w,
+                            dbias, B, workspace, workspace_bytes, ST(stream));
 }
 
 int b200rec_gather(const float* W, int64_t ldw, const int64_t* ids, float* out, int64_t n, int D,

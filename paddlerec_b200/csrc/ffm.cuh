@@ -212,8 +212,12 @@ struct FfmBwd {
     }
     return __ldg(dense + b * Dn + (m - F)) * __ldg(dense_w + (size_t)(m - F) * R + f * D + j);
   }
+  // Per (id, column) state the scheduling kernels compute once per segment before walking its
+  // positions; FFM's contribution needs none.
+  struct Col {};
+  __device__ __forceinline__ Col column(int /*p*/, int /*c*/) const { return {}; }
   // contribution of position p = b*F + f to column c of its gradient row
-  __device__ __forceinline__ float contrib(int p, int c) const {
+  __device__ __forceinline__ float contrib(int p, int c, Col) const {
     const int64_t b = p / F;
     const int f = p - (int)b * F;
     if (c < R) {
@@ -223,6 +227,18 @@ struct FfmBwd {
     }
     return c == R ? __ldg(gy1 + b) : 0.f;
   }
+  // Dense-parameter columns: [ddense_w (Dn*R) | ddense_w1 (Dn) | dbias].  Each adds sample b to acc.
+  __device__ __forceinline__ int w1_cols() const { return Dn; }
+  __device__ __forceinline__ float dense_w_acc(float acc, int64_t b, int k, int c) const {
+    const int m = c / D, j = c - m * D;
+    if (m == F + k) return acc;
+    const float s = __ldg(gy2 + b) * __ldg(dense + b * Dn + k);
+    return fmaf(s, partner(b, m, F + k, j), acc);
+  }
+  __device__ __forceinline__ float w1_acc(float acc, int64_t b, int k) const {
+    return fmaf(__ldg(gy1 + b), __ldg(dense + b * Dn + k), acc);
+  }
+  __device__ __forceinline__ float bias_acc(float acc, int64_t b) const { return acc + __ldg(gy1 + b); }
 };
 
 constexpr int kFfmHotChunk = 1024;   // positions per hot work item (one CTA)
@@ -248,9 +264,10 @@ struct FfmBwdWs {
 
 // One warp per distinct id: walks its sorted positions 32 columns at a time (fixed order per
 // column).  Ids with more than kHotThreshold positions are deferred to the hot kernel as
-// ceil(len / kFfmHotChunk) work items.
+// ceil(len / kFfmHotChunk) work items.  A is the per-position functor (FfmBwd, FatBwd).
+template <class A>
 __global__ void __launch_bounds__(kFfmThreads)
-ffm_bwd_light_kernel(FfmBwd a, const int32_t* __restrict__ seg_offsets,
+ffm_bwd_light_kernel(A a, const int32_t* __restrict__ seg_offsets,
                      const int32_t* __restrict__ sorted_pos, const int32_t* __restrict__ num_unique,
                      float* __restrict__ rows, int64_t ld_rows, int32_t* __restrict__ counters,
                      int32_t* __restrict__ items) {
@@ -278,7 +295,8 @@ ffm_bwd_light_kernel(FfmBwd a, const int32_t* __restrict__ seg_offsets,
       const int c = c0 + lane;
       float acc = 0.f;
       if (c < a.G) {
-        for (int i = beg; i < end; ++i) acc += a.contrib(sorted_pos[i], c);
+        const typename A::Col col = a.column(sorted_pos[beg], c);
+        for (int i = beg; i < end; ++i) acc += a.contrib(sorted_pos[i], c, col);
       }
       if (c < ld_rows) out[c] = acc;
     }
@@ -288,8 +306,9 @@ ffm_bwd_light_kernel(FfmBwd a, const int32_t* __restrict__ seg_offsets,
 // One CTA per hot work item: warp w takes positions beg+w, beg+w+8, ...; the 8 warp sums of a
 // column meet in warp order.  A single-chunk id writes its row; the chunks of a longer id write
 // partial rows that the combine kernel adds in chunk order.
+template <class A>
 __global__ void __launch_bounds__(kFfmThreads)
-ffm_bwd_hot_kernel(FfmBwd a, const int32_t* __restrict__ seg_offsets,
+ffm_bwd_hot_kernel(A a, const int32_t* __restrict__ seg_offsets,
                    const int32_t* __restrict__ sorted_pos, const int32_t* __restrict__ counters,
                    const int32_t* __restrict__ items, float* __restrict__ partials,
                    float* __restrict__ rows, int64_t ld_rows) {
@@ -309,7 +328,8 @@ ffm_bwd_hot_kernel(FfmBwd a, const int32_t* __restrict__ seg_offsets,
       const int c = c0 + lane;
       float acc = 0.f;
       if (c < a.G) {
-        for (int i = beg + warp; i < end; i += WPB) acc += a.contrib(sorted_pos[i], c);
+        const typename A::Col col = a.column(sorted_pos[beg], c);
+        for (int i = beg + warp; i < end; i += WPB) acc += a.contrib(sorted_pos[i], c, col);
       }
       s_acc[warp][lane] = acc;
       __syncthreads();
@@ -344,11 +364,13 @@ __global__ void ffm_bwd_combine_kernel(const int32_t* __restrict__ counters,
   }
 }
 
-// Dense-parameter gradients: thread = one output column q of [ddense_w (Dn*R) | ddense_w1 (Dn) |
-// dbias], blockIdx.y = a slice of the batch; each slice writes one partial row.
+// Dense-parameter gradients: thread = one output column q of [ddense_w (Dn*R) | w1 part
+// (a.w1_cols()) | dbias], blockIdx.y = a slice of the batch; each slice writes one partial row.
+template <class A>
 __global__ void __launch_bounds__(kFfmThreads)
-ffm_bwd_dense_kernel(FfmBwd a, int64_t B, int per_slice, float* __restrict__ partials) {
-  const int len = a.Dn * a.R + a.Dn + 1;
+ffm_bwd_dense_kernel(A a, int64_t B, int per_slice, float* __restrict__ partials) {
+  const int n1 = a.w1_cols();
+  const int len = a.Dn * a.R + n1 + 1;
   const int q = blockIdx.x * kFfmThreads + threadIdx.x;
   if (q >= len) return;
   const int64_t b0 = (int64_t)blockIdx.y * per_slice;
@@ -356,38 +378,75 @@ ffm_bwd_dense_kernel(FfmBwd a, int64_t B, int per_slice, float* __restrict__ par
   float acc = 0.f;
   if (q < a.Dn * a.R) {
     const int k = q / a.R, c = q - k * a.R;
-    const int m = c / a.D, j = c - m * a.D;
-    if (m != a.F + k) {
 #pragma unroll 4
-      for (int64_t b = b0; b < b1; ++b) {
-        const float s = __ldg(a.gy2 + b) * __ldg(a.dense + b * a.Dn + k);
-        acc = fmaf(s, a.partner(b, m, a.F + k, j), acc);
-      }
-    }
-  } else if (q < a.Dn * a.R + a.Dn) {
+    for (int64_t b = b0; b < b1; ++b) acc = a.dense_w_acc(acc, b, k, c);
+  } else if (q < a.Dn * a.R + n1) {
     const int k = q - a.Dn * a.R;
-    for (int64_t b = b0; b < b1; ++b) acc = fmaf(__ldg(a.gy1 + b), __ldg(a.dense + b * a.Dn + k), acc);
+    for (int64_t b = b0; b < b1; ++b) acc = a.w1_acc(acc, b, k);
   } else {
-    for (int64_t b = b0; b < b1; ++b) acc += __ldg(a.gy1 + b);
+    for (int64_t b = b0; b < b1; ++b) acc = a.bias_acc(acc, b);
   }
   partials[(size_t)blockIdx.y * len + q] = acc;
 }
 
-// out[q] = sum over slices of partials[slice][q], slices added in order.
+// out[q] = sum over slices of partials[slice][q], slices added in order.  n1 = the w1 part's
+// width (Dn for FFM, 0 for a model without dense_w1).
 __global__ void ffm_bwd_dense_reduce_kernel(const float* __restrict__ partials, int slices, int Dn,
-                                            int R, float* __restrict__ ddense_w,
+                                            int R, int n1, float* __restrict__ ddense_w,
                                             float* __restrict__ ddense_w1, float* __restrict__ dbias) {
-  const int len = Dn * R + Dn + 1;
+  const int len = Dn * R + n1 + 1;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= len) return;
   float t = 0.f;
   for (int s = 0; s < slices; ++s) t += partials[(size_t)s * len + q];
   if (q < Dn * R)
     ddense_w[q] = t;
-  else if (q < Dn * R + Dn)
+  else if (q < Dn * R + n1)
     ddense_w1[q - Dn * R] = t;
   else if (dbias != nullptr)
     *dbias = t;
+}
+
+// The backward's launch sequence over the grouping of the B*F ids: light warps, then (when some id
+// may be hot) the hot CTAs and the chunk combine, then the sliced dense-parameter partials and their
+// reduce.  The functor a decides what each position contributes; n1 is its w1 part's width.
+template <class A>
+static int run_ffm_bwd_schedule(const A& a, const FfmBwdWs& L, int64_t B, int n1,
+                                const int32_t* seg_offsets, const int32_t* sorted_pos,
+                                const int32_t* num_unique, float* dW_rows, int64_t ld_dw,
+                                float* ddense_w, float* ddense_w1, float* dbias, void* ws,
+                                cudaStream_t st) {
+  unsigned char* base = static_cast<unsigned char*>(ws);
+  int32_t* counters = reinterpret_cast<int32_t*>(base);
+  int32_t* items = reinterpret_cast<int32_t*>(base + L.off_items);
+  float* partials = reinterpret_cast<float*>(base + L.off_part);
+  float* dense_part = reinterpret_cast<float*>(base + L.off_dense);
+  const int Dn = a.Dn, R = a.R;
+
+  B200_CUDA(cudaMemsetAsync(counters, 0, 16, st));
+  const int64_t n = B * a.F;
+  constexpr int WPB = kFfmThreads / 32;
+  const unsigned lgrid = (unsigned)min((n + WPB - 1) / WPB, (int64_t)sm_count() * 16);
+  ffm_bwd_light_kernel<A><<<lgrid, kFfmThreads, 0, st>>>(a, seg_offsets, sorted_pos, num_unique,
+                                                         dW_rows, ld_dw, counters, items);
+  B200_LAUNCH_CHECK();
+  if (n > kHotThreshold) {
+    const unsigned hgrid = (unsigned)min(L.max_items, (int64_t)sm_count() * 8);
+    ffm_bwd_hot_kernel<A><<<hgrid, kFfmThreads, 0, st>>>(a, seg_offsets, sorted_pos, counters,
+                                                         items, partials, dW_rows, ld_dw);
+    B200_LAUNCH_CHECK();
+    ffm_bwd_combine_kernel<<<hgrid, 256, 0, st>>>(counters, items, partials, dW_rows, ld_dw, a.G);
+    B200_LAUNCH_CHECK();
+  }
+  const int len = Dn * R + n1 + 1;
+  const int per_slice = (int)((B + L.slices - 1) / L.slices);
+  const dim3 dgrid((unsigned)((len + kFfmThreads - 1) / kFfmThreads), (unsigned)L.slices);
+  ffm_bwd_dense_kernel<A><<<dgrid, kFfmThreads, 0, st>>>(a, B, per_slice, dense_part);
+  B200_LAUNCH_CHECK();
+  ffm_bwd_dense_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, st>>>(
+      dense_part, L.slices, Dn, R, n1, ddense_w, ddense_w1, dbias);
+  B200_LAUNCH_CHECK();
+  return B200REC_OK;
 }
 
 static int launch_ffm_bwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
@@ -418,37 +477,9 @@ static int launch_ffm_bwd(const float* W, int64_t ldw, const int64_t* ids, const
     if (dbias != nullptr) B200_CUDA(cudaMemsetAsync(dbias, 0, sizeof(float), st));
     return B200REC_OK;
   }
-  unsigned char* base = static_cast<unsigned char*>(ws);
-  int32_t* counters = reinterpret_cast<int32_t*>(base);
-  int32_t* items = reinterpret_cast<int32_t*>(base + L.off_items);
-  float* partials = reinterpret_cast<float*>(base + L.off_part);
-  float* dense_part = reinterpret_cast<float*>(base + L.off_dense);
   const FfmBwd a{W, ldw, ids, dense, dense_w, gy1, gy2, F, Dn, D, R, G, V, pad};
-
-  B200_CUDA(cudaMemsetAsync(counters, 0, 16, st));
-  const int64_t n = B * F;
-  constexpr int WPB = kFfmThreads / 32;
-  const unsigned lgrid = (unsigned)min((n + WPB - 1) / WPB, (int64_t)sm_count() * 16);
-  ffm_bwd_light_kernel<<<lgrid, kFfmThreads, 0, st>>>(a, seg_offsets, sorted_pos, num_unique,
-                                                      dW_rows, ld_dw, counters, items);
-  B200_LAUNCH_CHECK();
-  if (n > kHotThreshold) {
-    const unsigned hgrid = (unsigned)min(L.max_items, (int64_t)sm_count() * 8);
-    ffm_bwd_hot_kernel<<<hgrid, kFfmThreads, 0, st>>>(a, seg_offsets, sorted_pos, counters, items,
-                                                      partials, dW_rows, ld_dw);
-    B200_LAUNCH_CHECK();
-    ffm_bwd_combine_kernel<<<hgrid, 256, 0, st>>>(counters, items, partials, dW_rows, ld_dw, G);
-    B200_LAUNCH_CHECK();
-  }
-  const int len = Dn * R + Dn + 1;
-  const int per_slice = (int)((B + L.slices - 1) / L.slices);
-  const dim3 dgrid((unsigned)((len + kFfmThreads - 1) / kFfmThreads), (unsigned)L.slices);
-  ffm_bwd_dense_kernel<<<dgrid, kFfmThreads, 0, st>>>(a, B, per_slice, dense_part);
-  B200_LAUNCH_CHECK();
-  ffm_bwd_dense_reduce_kernel<<<(unsigned)((len + 255) / 256), 256, 0, st>>>(
-      dense_part, L.slices, Dn, R, ddense_w, ddense_w1, dbias);
-  B200_LAUNCH_CHECK();
-  return B200REC_OK;
+  return run_ffm_bwd_schedule(a, L, B, Dn, seg_offsets, sorted_pos, num_unique, dW_rows, ld_dw,
+                              ddense_w, ddense_w1, dbias, ws, st);
 }
 
 }  // namespace b200rec

@@ -244,7 +244,12 @@ class FusedTable(tnn.Module):
 
     state_dict() still exposes the reference's two keys (`embedding.weight` [V,D] and
     `embedding_one.weight` [V,1], as views of the slot array) and loads from them, so checkpoints
-    stay interchangeable.  The gradient is one SelectedRows of width D+1 (+pad) on `weight`."""
+    stay interchangeable.  The gradient is one SelectedRows of width D+1 (+pad) on `weight`.
+
+    With one name (`names=("embedding.weight",)`) the slot holds a single table [D emb | 0 | pad]
+    in the same layout, so the FFM-family kernels read it unchanged: the w1 column starts at zero,
+    its gradient column is always zero, and views, state_dict and grad_dense show only the
+    embedding."""
 
     def __init__(self, num_embeddings, embedding_dim, padding_idx=None, init_std=None, device=None,
                  names=("embedding.weight", "embedding_one.weight"), attr="_fused",
@@ -266,7 +271,8 @@ class FusedTable(tnn.Module):
         w = torch.zeros(num_embeddings, self.slot, device=device)
         std = init_std or 1.0
         if num_embeddings > 0:
-            tnn.init.trunc_normal_(w[:, :D + 1], 0.0, std, -2.0 * std, 2.0 * std)
+            ncols = D + 1 if len(names) == 2 else D
+            tnn.init.trunc_normal_(w[:, :ncols], 0.0, std, -2.0 * std, 2.0 * std)
             if padding_idx is not None:
                 w[padding_idx].zero_()
         self.weight = tnn.Parameter(w, requires_grad=False)
@@ -290,9 +296,10 @@ class FusedTable(tnn.Module):
         return -1 if self.padding_idx is None else int(self.padding_idx)
 
     def views(self):
+        """One view per name: (embedding [V,D], embedding_one [V,1]) or (embedding,)."""
         w = self.weight.detach()
         D = self.embedding_dim
-        return w[:, :D], w[:, D:D + 1]
+        return (w[:, :D], w[:, D:D + 1])[:len(self._names)]
 
     # ---- gradient sink protocol used by ops._EmbedFM -----------------------------------------
     def groups_for(self, ids, V, pad):
@@ -310,23 +317,22 @@ class FusedTable(tnn.Module):
         return self.weight.grad_rows
 
     def grad_dense(self):
-        """(dW [V,D], dW1 [V,1]) as dense tensors (tests / small tables)."""
+        """(dW [V,D], dW1 [V,1]), or (dW,) with one name, as dense tensors (tests / small tables)."""
         D = self.embedding_dim
         if self.weight.grad_rows is None:
             z = torch.zeros(self.num_embeddings, D + 1, device=self.weight.device)
         else:
             z = self.weight.grad_rows.to_dense()
-        return z[:, :D], z[:, D:D + 1]
+        return (z[:, :D], z[:, D:D + 1])[:len(self._names)]
 
     # ---- reference-compatible checkpoint keys -------------------------------------------------
     def _parent_prefix(self, prefix: str) -> str:
         return prefix[:-(len(self._attr) + 1)]
 
     def _save_to_state_dict(self, destination, prefix, keep_vars):
-        e, e1 = self.views()
         parent = self._parent_prefix(prefix)
-        destination[parent + self._names[0]] = e
-        destination[parent + self._names[1]] = e1
+        for name, view in zip(self._names, self.views()):
+            destination[parent + name] = view
 
     def _load_from_state_dict(self, *args, **kwargs):
         pass  # the owning module routes the reference-named keys here (load_views)
@@ -335,9 +341,8 @@ class FusedTable(tnn.Module):
         """Copy `<parent>embedding.weight` / `<parent>embedding_one.weight` into the slot array and
         return the state_dict without those keys (torch only hands a child the keys under ITS
         prefix, so the parent module calls this from its own _load_from_state_dict)."""
-        e, e1 = self.views()
         rest = dict(state_dict)
-        for name, view in ((self._names[0], e), (self._names[1], e1)):
+        for name, view in zip(self._names, self.views()):
             key = parent_prefix + name
             if key in rest:
                 with torch.no_grad():

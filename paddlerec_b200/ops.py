@@ -41,7 +41,8 @@ def _req(t: torch.Tensor, dtype, name: str) -> torch.Tensor:
 # it as `gpu_launches`.  KERNELS_PER_CALL is the static number of our kernels each entry point runs.
 LAUNCHES = 0
 KERNELS_PER_CALL = {
-    "embed_fm_fwd": 1, "group_ids": 3, "embed_fm_bwd": 5, "ffm_fwd": 1, "ffm_bwd": 5, "gather": 1, "segment_reduce": 3,
+    "embed_fm_fwd": 1, "group_ids": 3, "embed_fm_bwd": 5, "ffm_fwd": 1, "ffm_bwd": 5, "fat_ffm_pool_fwd": 1,
+    "fat_ffm_fwd": 1, "fat_ffm_bwd_attn": 1, "fat_ffm_bwd": 5, "gather": 1, "segment_reduce": 3,
     "shard_gather_push": 1, "shard_push_rows": 1, "shard_fm_grads_push": 1, "rows_to_dense": 1, "sparse_sgd": 1, "sparse_adam": 1, "sparse_adagrad": 1, "cross_v2_fwd": 1,
     "cross_v2_bwd": 2, "shard_bucketize": 2, "tower_split": 1, "tower_relu_bwd_split": 2,
     "tower_prep_weight": 1, "tower_fold_dw": 1, "tc_split": 1, "tc_split_bwd": 2,
@@ -330,6 +331,113 @@ def raw_ffm_bwd(W, ids, dense, dense_w, gy1, gy2, groups: "IdGroups", padding_id
                               D, V, int(padding_idx), ptr(ws), ws.numel(), _stream()), "ffm_bwd")
     _count("ffm_bwd")
     return dW_rows, ddense_w, ddense_w1, dbias
+
+
+def _fat_shapes(W, ids, dense, dense_w, D):
+    B, F = ids.shape
+    Dn = dense.shape[1]
+    NF = F + Dn
+    assert dense.shape[0] == B and dense_w.numel() == Dn * NF * D
+    return B, F, Dn, NF, NF * (NF - 1) // 2
+
+
+def raw_fat_ffm_pool_fwd(W, ids, dense, dense_w, padding_idx: int, D: int):
+    """CENet's max pool over FAT-DeepFFM's field-aware blocks (b200rec_fat_ffm_pool_fwd).  W: [V, ldw]
+    fused rows [R emb | w1 | pad] with R = (F + Dn) * D (w1 unused); dense_w [Dn, R].
+    Returns pool [B, NF*NF]; counts padding / out-of-range ids."""
+    lib = _lib.load()
+    W = _req(W, torch.float32, "W")
+    ids = _req(ids, torch.int64, "ids")
+    dense = _req(dense, torch.float32, "dense")
+    dense_w = _req(dense_w, torch.float32, "dense_w")
+    B, F, Dn, NF, _ = _fat_shapes(W, ids, dense, dense_w, D)
+    V, ldw = W.shape
+    pool = torch.empty(B, NF * NF, dtype=torch.float32, device=W.device)
+    check(lib.b200rec_fat_ffm_pool_fwd(ptr(W), ldw, ptr(ids), ptr(dense), ptr(dense_w), ptr(pool), B,
+                                       F, Dn, D, V, int(padding_idx), _stream()), "fat_ffm_pool_fwd")
+    _count("fat_ffm_pool_fwd")
+    return pool
+
+
+def raw_fat_ffm_fwd(W, ids, dense, dense_w, attn, bias, padding_idx: int, D: int):
+    """FAT-DeepFFM's attention-weighted first-order sum and Hadamard interaction
+    (b200rec_fat_ffm_fwd).  attn [B, NF*NF]; bias [1] or None (added to y1).
+    Returns (y1 [B], h [B, P*D])."""
+    lib = _lib.load()
+    W = _req(W, torch.float32, "W")
+    ids = _req(ids, torch.int64, "ids")
+    dense = _req(dense, torch.float32, "dense")
+    dense_w = _req(dense_w, torch.float32, "dense_w")
+    attn = _req(attn, torch.float32, "attn")
+    if bias is not None:
+        bias = _req(bias, torch.float32, "bias")
+    B, F, Dn, NF, P = _fat_shapes(W, ids, dense, dense_w, D)
+    assert attn.shape == (B, NF * NF)
+    V, ldw = W.shape
+    y1 = torch.empty(B, dtype=torch.float32, device=W.device)
+    h = torch.empty(B, P * D, dtype=torch.float32, device=W.device)
+    check(lib.b200rec_fat_ffm_fwd(ptr(W), ldw, ptr(ids), ptr(dense), ptr(dense_w), ptr(attn),
+                                  ptr(bias), ptr(y1), ptr(h), B, F, Dn, D, V, int(padding_idx),
+                                  _stream()), "fat_ffm_fwd")
+    _count("fat_ffm_fwd")
+    return y1, h
+
+
+def raw_fat_ffm_bwd_attn(W, ids, dense, dense_w, attn, gy1, dh, padding_idx: int, D: int):
+    """dL/dattn of raw_fat_ffm_fwd from gy1 [B] and dh [B, P*D] (b200rec_fat_ffm_bwd_attn)."""
+    lib = _lib.load()
+    W = _req(W, torch.float32, "W")
+    ids = _req(ids, torch.int64, "ids")
+    dense = _req(dense, torch.float32, "dense")
+    dense_w = _req(dense_w, torch.float32, "dense_w")
+    attn = _req(attn, torch.float32, "attn")
+    gy1 = _req(gy1, torch.float32, "gy1").reshape(-1)
+    dh = _req(dh, torch.float32, "dh")
+    B, F, Dn, NF, P = _fat_shapes(W, ids, dense, dense_w, D)
+    assert attn.shape == (B, NF * NF) and dh.shape == (B, P * D) and gy1.numel() == B
+    V, ldw = W.shape
+    dattn = torch.empty(B, NF * NF, dtype=torch.float32, device=W.device)
+    check(lib.b200rec_fat_ffm_bwd_attn(ptr(W), ldw, ptr(ids), ptr(dense), ptr(dense_w), ptr(attn),
+                                       ptr(gy1), ptr(dh), ptr(dattn), B, F, Dn, D, V,
+                                       int(padding_idx), _stream()), "fat_ffm_bwd_attn")
+    _count("fat_ffm_bwd_attn")
+    return dattn
+
+
+def raw_fat_ffm_bwd(W, ids, dense, dense_w, attn, gy1, dh, dpool, groups: "IdGroups",
+                    padding_idx: int, D: int):
+    """Table and dense-parameter gradients of FAT-DeepFFM through the attention product and the max
+    pool (b200rec_fat_ffm_bwd).  Returns (dW_rows [min(B*F, V), G] = [R emb | zeros] with
+    G = fused_grad_cols(R), only the first groups.num[0] rows valid; ddense_w [Dn, R]; dbias [1])."""
+    lib = _lib.load()
+    W = _req(W, torch.float32, "W")
+    ids = _req(ids, torch.int64, "ids")
+    dense = _req(dense, torch.float32, "dense")
+    dense_w = _req(dense_w, torch.float32, "dense_w")
+    attn = _req(attn, torch.float32, "attn")
+    gy1 = _req(gy1, torch.float32, "gy1").reshape(-1)
+    dh = _req(dh, torch.float32, "dh")
+    dpool = _req(dpool, torch.float32, "dpool")
+    B, F, Dn, NF, P = _fat_shapes(W, ids, dense, dense_w, D)
+    assert attn.shape == dpool.shape == (B, NF * NF) and dh.shape == (B, P * D)
+    V, ldw = W.shape
+    R = NF * D
+    G = fused_grad_cols(R)
+    dev = W.device
+    nbytes = ctypes.c_size_t(0)
+    check(lib.b200rec_fat_ffm_bwd_workspace_bytes(B, F, Dn, D, ctypes.byref(nbytes)),
+          "fat_ffm_bwd_ws")
+    ws = workspace(nbytes.value, dev, "fat_ffm_bwd")
+    dW_rows = torch.empty(max(min(B * F, V), 1), G, dtype=torch.float32, device=dev)
+    ddense_w = torch.empty(Dn, R, dtype=torch.float32, device=dev)
+    dbias = torch.empty(1, dtype=torch.float32, device=dev)
+    check(lib.b200rec_fat_ffm_bwd(ptr(W), ldw, ptr(ids), ptr(dense), ptr(dense_w), ptr(attn),
+                                  ptr(gy1), ptr(dh), ptr(dpool), ptr(groups.seg_offsets),
+                                  ptr(groups.sorted_pos), ptr(groups.num), ptr(dW_rows), G,
+                                  ptr(ddense_w), ptr(dbias), B, F, Dn, D, V, int(padding_idx),
+                                  ptr(ws), ws.numel(), _stream()), "fat_ffm_bwd")
+    _count("fat_ffm_bwd")
+    return dW_rows, ddense_w, dbias
 
 
 def raw_gather(W: torch.Tensor, ids: torch.Tensor, padding_idx: int,
@@ -960,6 +1068,92 @@ def ffm(W, ids, dense, dense_w, dense_w1, bias, padding_idx, sink, D):
     return _FFM.apply(W, ids, dense, dense_w, dense_w1, bias, padding_idx, sink, D)
 
 
+class FatLink:
+    """What FAT-DeepFFM's two autograd halves share in one step: the gather's inputs, and what
+    _FatInteract.backward leaves for _FatPool.backward, so the table gradient is ONE pass over the
+    ids (kernel b200rec_fat_ffm_bwd) that sees both of its routes."""
+
+    def __init__(self, W, ids, dense, dense_w, padding_idx, sink, D):
+        self.W, self.ids, self.dense, self.padding_idx, self.sink, self.D = (
+            W, ids, dense, padding_idx, sink, D)
+        B, Dn = dense.shape
+        self.NF = ids.shape[1] + Dn
+        self.dense_w = dense_w.reshape(Dn, self.NF * D)
+        self.gy1 = self.dh = self.attn = None
+
+
+class _FatPool(torch.autograd.Function):
+    """CENLayer's gather and max pool (fat_deepffm/net.py:107-132).  Its backward runs after
+    _FatInteract's (the pool reaches the interaction only through the attention MLP) and takes the
+    whole table, dense_w and bias gradient in one kernel; dense_w and bias are inputs here for
+    that reason, although only the interaction adds the bias."""
+
+    @staticmethod
+    def forward(ctx, dense_w, bias, link):
+        pool = raw_fat_ffm_pool_fwd(link.W, link.ids, link.dense, link.dense_w, link.padding_idx,
+                                    link.D)
+        ctx.link = link
+        ctx.dense_w_shape = dense_w.shape
+        ctx.bias_shape = None if bias is None else bias.shape
+        return pool
+
+    @staticmethod
+    def backward(ctx, dpool):
+        k = ctx.link
+        B = k.ids.shape[0]
+        P = k.NF * (k.NF - 1) // 2
+        dev = k.dense.device
+        gy1 = k.gy1 if k.gy1 is not None else torch.zeros(B, device=dev)
+        dh = k.dh if k.dh is not None else torch.zeros(B, P * k.D, device=dev)
+        attn = k.attn if k.attn is not None else torch.zeros(B, k.NF * k.NF, device=dev)
+        k.gy1 = k.dh = k.attn = None
+        V = k.W.shape[0]
+        groups = k.sink.groups_for(k.ids, V, k.padding_idx)
+        dW_rows, ddense_w, dbias = raw_fat_ffm_bwd(k.W, k.ids, k.dense, k.dense_w, attn, gy1, dh,
+                                                   dpool.contiguous(), groups, k.padding_idx, k.D)
+        k.sink.accept_fused(SelectedRows(groups.unique_ids, dW_rows, groups.num, V))
+        db = None if ctx.bias_shape is None else dbias.reshape(ctx.bias_shape)
+        return ddense_w.reshape(ctx.dense_w_shape), db, None
+
+
+class _FatInteract(torch.autograd.Function):
+    """The attention product, first-order sum and field-aware Hadamard pairs
+    (fat_deepffm/net.py:144-149, 219-251) plus the layer's bias.  Its backward returns dattn and
+    leaves gy1, dh and attn on the link for _FatPool.backward."""
+
+    @staticmethod
+    def forward(ctx, attn, bias, link):
+        y1, h = raw_fat_ffm_fwd(link.W, link.ids, link.dense, link.dense_w, attn, bias,
+                                link.padding_idx, link.D)
+        ctx.save_for_backward(attn)
+        ctx.link = link
+        return y1.unsqueeze(1), h
+
+    @staticmethod
+    def backward(ctx, dy1, dh):
+        (attn,) = ctx.saved_tensors
+        k = ctx.link
+        B = attn.shape[0]
+        P = k.NF * (k.NF - 1) // 2
+        gy1 = (dy1.reshape(-1).contiguous() if dy1 is not None
+               else torch.zeros(B, device=attn.device))
+        dh = dh.contiguous() if dh is not None else torch.zeros(B, P * k.D, device=attn.device)
+        dattn = raw_fat_ffm_bwd_attn(k.W, k.ids, k.dense, k.dense_w, attn, gy1, dh, k.padding_idx,
+                                     k.D)
+        k.gy1, k.dh, k.attn = gy1, dh, attn.contiguous()
+        return dattn, None, None
+
+
+def fat_ffm_pool(link: FatLink, dense_w, bias):
+    """-> pool [B, NF*NF] (CENet's AdaptiveMaxPool1D over every field-aware block)."""
+    return _FatPool.apply(dense_w, bias, link)
+
+
+def fat_ffm_interact(link: FatLink, attn, bias):
+    """-> (y1 [B,1] with bias added, h [B, P*D]) from the attention weights attn [B, NF*NF]."""
+    return _FatInteract.apply(attn, bias, link)
+
+
 def fused_grad_cols(D: int) -> int:
     """Columns of a fused gradient row [D | g1 | pad]: D+1 rounded up to a multiple of 4."""
     return (D + 1 + 3) // 4 * 4
@@ -1505,7 +1699,8 @@ def _wrap_timed(fn, name):
     return timed
 
 
-for _n in ("group_ids", "embed_fm_bwd", "ffm_fwd", "ffm_bwd", "gather", "gather_pool_sum", "segment_reduce", "sparse_sgd",
+for _n in ("group_ids", "embed_fm_bwd", "ffm_fwd", "ffm_bwd", "fat_ffm_pool_fwd", "fat_ffm_fwd",
+           "fat_ffm_bwd_attn", "fat_ffm_bwd", "gather", "gather_pool_sum", "segment_reduce", "sparse_sgd",
            "sparse_adam", "sparse_adagrad", "cross_v2_fwd", "cross_v2_bwd", "shard_bucketize",
            "shard_gather_push", "shard_push_rows", "shard_fm_grads_push",
            "tc_split", "tc_split_bwd", "tc_prep_weight", "tc_linear_fwd", "tc_cross_fwd",
