@@ -151,12 +151,13 @@ int b200rec_fat_ffm_pool_fwd(const float* W, int64_t ldw, const int64_t* ids, co
 /* With attn [B, NF*NF] and s[b,n,m,:] = attn[b, n*NF+m] * e[b,n, m*D:(m+1)*D]:
  *   y1[b] = sum_{n,m,d} s[b,n,m,d] (+ bias[0] if bias != NULL), summed in a fixed order
  *   h[b, p(n,m)*D + d] = s[b,n,m,d] * s[b,m,n,d]   for n < m in row-major pair order
- * Nothing of size [B,NF,R] is written. */
+ * Nothing of size [B,NF,R] is written.  h may be NULL when P*D = 0 (one field: no pairs). */
 int b200rec_fat_ffm_fwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
                         const float* dense_w, const float* attn, const float* bias, float* y1,
                         float* h, int64_t B, int F, int Dn, int D, int64_t V, int64_t padding_idx,
                         void* stream);
-/* dattn[b, n*NF+m] = sum_d e[b,n,m*D+d] * (gy1[b] + [n != m] * dh[b, p(n,m)*D+d] * s[b,m,n,d]) */
+/* dattn[b, n*NF+m] = sum_d e[b,n,m*D+d] * (gy1[b] + [n != m] * dh[b, p(n,m)*D+d] * s[b,m,n,d])
+ * dh may be NULL when P*D = 0. */
 int b200rec_fat_ffm_bwd_attn(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
                              const float* dense_w, const float* attn, const float* gy1,
                              const float* dh, float* dattn, int64_t B, int F, int Dn, int D,
@@ -169,7 +170,7 @@ int b200rec_fat_ffm_bwd_attn(const float* W, int64_t ldw, const int64_t* ids, co
  *   ddense_w[k, c] = sum_b dense[b,k] * de(b, F+k, c);   dbias[0] = sum_b gy1[b] (may be NULL)
  * The argmax of a dense block is taken on the fp32 product dense * dense_w.  Only the first
  * num_unique[0] rows of dW_rows are written, so it needs min(B*F, V) rows.  Every sum has a fixed
- * order, no float atomics: a second run is bit-identical. */
+ * order, no float atomics: a second run is bit-identical.  dh may be NULL when P*D = 0. */
 int b200rec_fat_ffm_bwd_workspace_bytes(int64_t B, int F, int Dn, int D, size_t* bytes_host);
 int b200rec_fat_ffm_bwd(const float* W, int64_t ldw, const int64_t* ids, const float* dense,
                         const float* dense_w, const float* attn, const float* gy1, const float* dh,

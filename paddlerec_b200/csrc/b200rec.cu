@@ -190,7 +190,8 @@ int b200rec_fat_ffm_fwd(const float* W, int64_t ldw, const int64_t* ids, const f
                         void* stream) {
   B200_REQUIRE(B >= 0 && V > 0, "fat_ffm_fwd: bad sizes");
   if (B > 0) {
-    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(attn); NOT_NULL(y1); NOT_NULL(h);
+    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(attn); NOT_NULL(y1);
+    if (fat_pairs(F, Dn) * D > 0) NOT_NULL(h);     // one field: no pairs, h has no elements
     if (Dn > 0) { NOT_NULL(dense); NOT_NULL(dense_w); }
   }
   const FatSampleArgs a{W, ldw, ids, dense, dense_w, attn, bias, nullptr, nullptr, y1, h,
@@ -204,7 +205,8 @@ int b200rec_fat_ffm_bwd_attn(const float* W, int64_t ldw, const int64_t* ids, co
                              int64_t V, int64_t padding_idx, void* stream) {
   B200_REQUIRE(B >= 0 && V > 0, "fat_ffm_bwd_attn: bad sizes");
   if (B > 0) {
-    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(attn); NOT_NULL(gy1); NOT_NULL(dh); NOT_NULL(dattn);
+    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(attn); NOT_NULL(gy1); NOT_NULL(dattn);
+    if (fat_pairs(F, Dn) * D > 0) NOT_NULL(dh);
     if (Dn > 0) { NOT_NULL(dense); NOT_NULL(dense_w); }
   }
   const FatSampleArgs a{W, ldw, ids, dense, dense_w, attn, nullptr, gy1, dh, nullptr, dattn,
@@ -230,9 +232,10 @@ int b200rec_fat_ffm_bwd(const float* W, int64_t ldw, const int64_t* ids, const f
   B200_REQUIRE(B >= 0 && V > 0, "fat_ffm_bwd: bad sizes");
   if (Dn > 0) NOT_NULL(ddense_w);
   if (B > 0) {
-    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(attn); NOT_NULL(gy1); NOT_NULL(dh); NOT_NULL(dpool);
+    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(attn); NOT_NULL(gy1); NOT_NULL(dpool);
     NOT_NULL(seg_offsets); NOT_NULL(sorted_pos); NOT_NULL(num_unique); NOT_NULL(dW_rows);
     NOT_NULL(workspace);
+    if (fat_pairs(F, Dn) * D > 0) NOT_NULL(dh);
     if (Dn > 0) { NOT_NULL(dense); NOT_NULL(dense_w); }
   }
   const int NF = F + Dn, R = NF * D;

@@ -22,6 +22,12 @@ __host__ __device__ inline int fat_pair_index(int n, int m, int NF) {   // n < m
   return n * NF - n * (n + 1) / 2 + (m - n - 1);
 }
 
+// P = NF(NF-1)/2 field pairs; 0 at NF = 1, where h and dh have no elements
+inline int64_t fat_pairs(int F, int Dn) {
+  const int64_t NF = (int64_t)F + Dn;
+  return NF * (NF - 1) / 2;
+}
+
 // ---- pool forward ------------------------------------------------------------------------------
 // One thread per (sample, block): a streaming gather in which each row is read once.  Padding and
 // out-of-range ids read as a zero row and are counted here (once per position), not by the

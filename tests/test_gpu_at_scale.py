@@ -24,6 +24,7 @@ import torch
 
 from oracle import nets
 from oracle import optim as ooptim
+from tests.test_gpu_fat_deepffm import _fat_smem, _gamma, _oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -57,12 +58,18 @@ FFM_THREADS = 256         # ffm.cuh:19  kFfmThreads
 FFM_MAX_FIELDS = 64       # ffm.cuh:20  kFfmMaxFields
 FFM_FWD_MAX_CTAS_PER_SM = 2048 // FFM_THREADS  # ffm.cuh:176-179 grid = min(B, SM*per_sm), per_sm from
 #                           the occupancy call: at most 2048 threads per SM
-FFM_HOT_CHUNK = 1024      # ffm.cuh:228 kFfmHotChunk; items pack c | (chunks << 16) :270
-FFM_MAX_CHUNKS = 32767    # ffm.cuh:406 B*F < 32767 * kFfmHotChunk
-FFM_MAX_SLICES = 256      # ffm.cuh:241 slices = min(256, ceil(B/256))
-FFM_LIGHT_CTAS_PER_SM = 16  # ffm.cuh:431 light grid min(ceil(n/8), 16*SM)
-FFM_HOT_CTAS_PER_SM = 8   # ffm.cuh:436 hot / combine grid min(max_items, 8*SM)
+FFM_HOT_CHUNK = 1024      # ffm.cuh:244 kFfmHotChunk; items pack c | (chunks << 16) :287
+FFM_MAX_CHUNKS = 32767    # ffm.cuh:465 B*F < 32767 * kFfmHotChunk
+FFM_MAX_SLICES = 256      # ffm.cuh:257 slices = min(256, ceil(B/256))
+FFM_LIGHT_CTAS_PER_SM = 16  # ffm.cuh:429 light grid min(ceil(n/8), 16*SM)
+FFM_HOT_CTAS_PER_SM = 8   # ffm.cuh:434 hot / combine grid min(max_items, 8*SM)
 WIDE_CTAS_PER_SM = 64     # gather_scatter.cuh:399, 428 wide-row grids min(ceil(n/8), 64*SM)
+FAT_POOL_THREADS = 256    # fat_ffm.cuh:322-324 pool grid min(ceil(B*NF^2/256), 16*SM) of 256 threads
+FAT_POOL_CTAS_PER_SM = 16
+FAT_SAMPLE_MAX_CTAS_PER_SM = 2048 // FFM_THREADS  # fat_ffm.cuh:350-353 grid = min(B, SM*per_sm),
+#                           per_sm from the occupancy call: at most 2048 threads per SM
+FAT_MAX_POSITIONS = FFM_MAX_CHUNKS * FFM_HOT_CHUNK  # fat_ffm.cuh:370 B*F < 32767 * kFfmHotChunk
+#                           FatSmem, fat_ffm.cuh:70-81, is mirrored by test_gpu_fat_deepffm._fat_smem
 
 
 def _ops():
@@ -1037,7 +1044,7 @@ def _ffm_bwd_ids(B, F, V, g):
 
 def ffm_bwd_chain(counts):
     """Longest fp32 chain of the columns < R of one gradient row, from its segment length
-    (ffm.cuh:249-345); every term g2 * partner is itself up to 2 roundings (a dense partner is
+    (ffm.cuh:265-365); every term g2 * partner is itself up to 2 roundings (a dense partner is
     x * dense_w).  Light (<= 64 positions): one lane adds the segment in order, len + 2.  Hot, one
     chunk: each of 8 warps adds ceil(len/8) positions, the 8 warp sums meet in order,
     ceil(len/8) + 8 + 2.  Several chunks: 1024/8 = 128 per warp, 8 warp sums, then the combine
@@ -1059,7 +1066,7 @@ def test_ffm_bwd_at_scale(Dn, D, B):
     element-wise against the per-position contributions g2[b] * e[b, m, block f] (m != f) and
     g1[b] merged in fp64 with index_add, bound ffm_bwd_chain(len) for columns < R and 2 less for
     column R (g1 terms are not rounded); columns R+1..G-1 must be exactly 0.
-    Dense gradients (ffm.cuh:349-391): each of the `slices` = min(256, ceil(B/256)) slices sums
+    Dense gradients (ffm.cuh:367-408): each of the `slices` = min(256, ceil(B/256)) slices sums
     per_slice samples with fmaf(g2*x, partner, acc) (+2 roundings per term, +1 for a dense partner's
     x*dense_w), then the slice partials are added in order: ddense_w k = per_slice + 3 + slices,
     ddense_w1 k = per_slice + 1 + slices, dbias k = per_slice + slices.  B = 65436 leaves the last
@@ -1159,8 +1166,8 @@ def test_ffm_bwd_at_scale(Dn, D, B):
 
 
 def test_ffm_bwd_chunk_packing_limit():
-    """Work items pack chunk | (chunks << 16) into one int32 (ffm.cuh:270), which the launcher
-    bounds by B*F < 32767*1024 (ffm.cuh:406).  At F=1, Dn=0, D=1 and B*F = 32767*1024 - 1, id 1
+    """Work items pack chunk | (chunks << 16) into one int32 (ffm.cuh:287), which the launcher
+    bounds by B*F < 32767*1024 (ffm.cuh:465).  At F=1, Dn=0, D=1 and B*F = 32767*1024 - 1, id 1
     takes 32766*1024 + 512 positions (32767 chunks: chunk index 32766, chunks << 16 =
     2,147,418,112), all with gy1 = 1.0; the other 511 positions go to distinct ids.  Each full chunk
     sums to exactly 1024 (8 warps of 128 ones), and every partial total of the combine is an even
@@ -1362,3 +1369,410 @@ def test_wide_row_optimizers_at_scale(case):
         assert_within(W_full[inner, cols][i], Wr, U * (2 * Wr.abs() + upd), "adagrad W " + case)
     assert outside_unchanged(W_full, W0_full), "adagrad W " + case
     assert outside_unchanged(g2_full, torch.zeros_like(g2_full)), "adagrad g2sum " + case
+
+
+# ================================================================================================
+# 13. FAT-DeepFFM (fat_ffm.cuh): max pool, persistent forward and dattn, FatBwd on FFM's backward
+# ================================================================================================
+def _fat_e(W, ids, dense, dense_w, s, e, D, pad):
+    """Samples s:e as E [b, NF, NF, D] in fp32, exactly as the kernels form it: E[b, n, m] is
+    block m of row n, i.e. of the table row (zero for padding and out-of-range ids) or of the
+    fp32 product dense * dense_w."""
+    V = W.shape[0]
+    F, Dn = ids.shape[1], dense.shape[1]
+    NF = F + Dn
+    idb = ids[s:e]
+    ok = ((idb >= 0) & (idb < V) & (idb != pad)).unsqueeze(2)
+    rows = torch.where(ok, W[idb.clamp(0, V - 1), :NF * D], 0.0)
+    return torch.cat([rows, dense[s:e].unsqueeze(2) * dense_w.unsqueeze(0)], 1).view(e - s, NF, NF, D)
+
+
+def _fat_closed_form(E32, attn, gy1, dh, dpool=None, bias=None):
+    """FAT-DeepFFM's interaction and its gradients in fp64, in closed form, for the samples of E32.
+    With A = attn as [b, NF, NF], ^T swapping n and m, DH = dh spread symmetrically with a zero
+    diagonal and `first` the one-hot of the first index where E equals its block maximum:
+        pool  = max_d E                          (fp32, exact)
+        y1    = sum A.E + bias
+        h     = (A.E)[n<m] . (A^T.E^T)[n<m]
+        dattn = sum_d E . (gy1 + DH.A^T.E^T)
+        de    = A.(gy1 + DH.A^T.E^T) + first.dpool      (only when dpool is given)
+    Returns (pool, values, magnitudes); the magnitudes are the same expressions on absolute values
+    (first unchanged): the sum of |terms| each output adds."""
+    b, NF, _, D = E32.shape
+    P = NF * (NF - 1) // 2
+    iu = torch.triu_indices(NF, NF, 1, device=DEV)
+    top = E32.amax(-1, keepdim=True)
+    pool = top.reshape(b, NF * NF)
+    if dpool is not None:
+        at = (E32 == top).to(torch.int8).argmax(-1, keepdim=True)
+        first = torch.zeros(E32.shape, dtype=torch.float64, device=DEV).scatter_(-1, at, 1.0)
+    out = []
+    for f in (lambda t: t.double(), lambda t: t.double().abs()):
+        E = f(E32)
+        A = f(attn).view(b, NF, NF, 1)
+        DH = torch.zeros(E.shape, dtype=torch.float64, device=DEV)
+        d = f(dh).view(b, P, D)
+        DH[:, iu[0], iu[1]] = d
+        DH[:, iu[1], iu[0]] = d
+        S = A * E
+        St = S.transpose(1, 2)
+        ds = f(gy1).view(b, 1, 1, 1) + DH * St
+        r = {"y1": S.sum((1, 2, 3)) + (0.0 if bias is None else f(bias)),
+             "h": (S[:, iu[0], iu[1]] * St[:, iu[0], iu[1]]).reshape(b, P * D),
+             "dattn": (E * ds).sum(3).reshape(b, NF * NF)}
+        if dpool is not None:
+            r["de"] = A * ds + first * f(dpool).view(b, NF, NF, 1)
+        out.append(r)
+    return pool, out[0], out[1]
+
+
+def _fat_chunk(NF, D):
+    return max(1, (1 << 22) // (NF * NF * D))
+
+
+def test_fat_closed_form_matches_autograd_oracle():
+    """The closed form above equals _oracle (autograd over the reference's operations) exactly, on
+    inputs quantised to multiples of 1/4 so that every fp64 sum is exact in any order.  Table
+    blocks hold ties, among them all-nonpositive blocks with both -0.0 and +0.0; dense values
+    include -0.0 and 0; padding and out-of-range ids are mixed in."""
+    B, F, Dn, D, V, pad = 300, 5, 3, 4, 50, 3
+    NF, R = F + Dn, (F + Dn) * D
+    g = torch.Generator(device=DEV).manual_seed(13)
+    q = lambda lo, hi, *s: torch.randint(lo, hi, s, generator=g, device=DEV) / 4  # noqa: E731
+    W = _ffm_table(V, R, g)
+    W[:, :R] = q(-8, 9, V, R)
+    W[:, R] = 7.0
+    W[::2, :D] = -q(1, 9, (V + 1) // 2, D)
+    W[::2, 1], W[::2, 3] = -0.0, 0.0
+    ids = torch.randint(0, V, (B, F), generator=g, device=DEV)
+    ids[::11, 0], ids[::13, 1], ids[::17, 2] = pad, -1, V + 2
+    dense = torch.tensor([-1, -0.5, -0.0, 0.0, 0.5, 1.0], device=DEV)[
+        torch.randint(0, 6, (B, Dn), generator=g, device=DEV)]
+    dense_w = q(-8, 9, Dn, R)
+    attn, gy1, dh, dpool = q(0, 5, B, NF * NF), q(-4, 5, B), q(-4, 5, B, NF * (NF - 1) // 2 * D), \
+        q(-4, 5, B, NF * NF)
+    bias = torch.tensor([0.25], device=DEV)
+    ties = W[:, :R].view(V, NF, D)
+    hit = (ties == ties.amax(-1, keepdim=True)).to(torch.int8)
+    assert bool((hit.argmax(-1) != D - 1 - hit.flip(-1).argmax(-1)).any()), "no tied table block"
+
+    pool, r, _ = _fat_closed_form(_fat_e(W, ids, dense, dense_w, 0, B, D, pad), attn, gy1, dh, dpool,
+                                  bias)
+    ref = _oracle(W, ids, dense, dense_w, attn, bias, gy1, dh, dpool, D, pad)
+    ok = ((ids >= 0) & (ids < V) & (ids != pad)).reshape(-1)
+    de = r["de"].reshape(B, NF, R)
+    dW = torch.zeros(V, R, dtype=torch.float64, device=DEV).index_add_(
+        0, ids.reshape(-1)[ok], de[:, :F].reshape(B * F, R)[ok])
+    ddw = torch.einsum("bk,bkr->kr", dense.double(), de[:, F:])
+    assert torch.equal(pool.double(), ref["pool"])
+    for k in ("y1", "h", "dattn"):
+        assert torch.equal(r[k], ref[k]), k
+    assert torch.equal(dW, ref["dW"]) and torch.equal(ddw, ref["ddw"])
+
+
+def _fat_sample_ids(B, F, V, pad, g):
+    """[B, F] ids over [1, V): 3% padding, 0.5% negative, 0.5% >= V."""
+    ids = torch.randint(1, V, (B, F), generator=g, device=DEV)
+    r = torch.rand(B, F, generator=g, device=DEV)
+    ids[r < 0.03] = pad
+    neg, big = (r >= 0.03) & (r < 0.035), (r >= 0.035) & (r < 0.04)
+    ids[neg] = -1 - torch.randint(0, 5, (B, F), generator=g, device=DEV)[neg]
+    ids[big] = V + torch.randint(0, 5, (B, F), generator=g, device=DEV)[big]
+    return ids
+
+
+@pytest.mark.parametrize("F,Dn,D,B,nbuf", [
+    (26, 13, 21, None, 2),     # the largest double-buffered shape at F=26, Dn=13
+    (26, 13, 22, None, 1),     # the smallest single-buffered one
+    (26, 13, 36, None, 1),     # the largest D that fits at all
+    (26, 13, 10, 65536, 2),    # the benchmark shape
+    (40, 24, 7, None, 2),      # NF = 64: 16 attention entries per thread, P = 2016 pairs
+    (26, 0, 10, None, 2),      # no dense fields
+    (1, 1, 3, None, 2),        # NF = 2: only B ~ 405k makes the pool's grid loop
+    (1, 0, 4, None, 2),        # NF = 1: P = 0, h and dh have no elements
+])
+def test_fat_sample_kernels_at_scale(F, Dn, D, B, nbuf):
+    """fat_ffm_pool_kernel and fat_ffm_sample_kernel<fwd / bwd>.  The pool runs one thread per
+    (sample, block) on min(ceil(B*NF^2/256), 16*SM) CTAs (fat_ffm.cuh:322-324); the sample kernels
+    run persistent CTAs, grid = min(B, SM*per_sm) with per_sm <= 8 (fat_ffm.cuh:350-353).  B
+    defaults to the larger of 3*8*SM + 17 and the pool's 3-pass size, so every CTA takes >= 3
+    samples (with two buffers, every CTA stages into both and prefetches across iterations) and
+    every pool thread >= 3 blocks.  The buffering each case gets is asserted from the FatSmem
+    mirror against the device's opt-in shared-memory limit.
+    Against _fat_closed_form, bounds as test_gpu_fat_deepffm._check_all derives them:
+    pool bit for bit; y1 gamma(ceil(NF^2/256)*(D+1) + 14) (per thread ceil(NF^2/256) blocks of D
+    adds and one fma, 5 shuffles, 8 warp sums, the bias); h gamma(5); dattn gamma(D+5).
+    Padding, negative and >= V ids read as zero rows; the pool counts each out-of-range position
+    once, fwd and bwd_attn count none.  The w1 column (7.0) and the slot padding (123.0) must not
+    leak.  A second run of each kernel is bit-identical."""
+    ops = _ops()
+    SM = _sm()
+    NF = F + Dn
+    R, P, NN = NF * D, NF * (NF - 1) // 2, NF * NF
+    limit = torch.cuda.get_device_properties(0).shared_memory_per_block_optin
+    if nbuf == 2:
+        assert _fat_smem(F, Dn, D, 2) <= limit, "F=%d Dn=%d D=%d no longer double-buffered" % (F, Dn, D)
+    else:
+        assert _fat_smem(F, Dn, D, 2) > limit >= _fat_smem(F, Dn, D, 1), \
+            "F=%d Dn=%d D=%d is no longer single-buffered" % (F, Dn, D)
+    if D == 36:
+        assert _fat_smem(F, Dn, D + 1, 1) > limit, "D=37 fits: D=36 is no longer the largest shape"
+    B = B or max(3 * FAT_SAMPLE_MAX_CTAS_PER_SM * SM + 17,
+                 _cdiv(3 * FAT_POOL_CTAS_PER_SM * SM * FAT_POOL_THREADS, NN))
+    what = "fat F=%d Dn=%d D=%d B=%d" % (F, Dn, D, B)
+    assert_loops("fat_ffm_sample_kernel %s (%d buffers): samples per CTA" % (what, nbuf),
+                 B // (FAT_SAMPLE_MAX_CTAS_PER_SM * SM))
+    pgrid = min(_cdiv(B * NN, FAT_POOL_THREADS), FAT_POOL_CTAS_PER_SM * SM)
+    assert_loops("fat_ffm_pool_kernel %s: blocks per thread" % what, B * NN // (pgrid * FAT_POOL_THREADS))
+    V, pad = 20_000, 0
+    g = torch.Generator(device=DEV).manual_seed(1000 * D + NF)
+    W = _ffm_table(V, R, g)
+    W[:, R] = 7.0
+    ids = _fat_sample_ids(B, F, V, pad, g)
+    n_oob = int(((ids < 0) | (ids >= V)).sum())
+    assert n_oob > 0 and int((ids == pad).sum()) > 0
+    dense = torch.rand(B, Dn, generator=g, device=DEV) * 2 - 0.5
+    dense_w = torch.randn(Dn, R, generator=g, device=DEV) * 0.1
+    attn = torch.relu(torch.randn(B, NN, generator=g, device=DEV) + 0.3)
+    gy1 = torch.randn(B, generator=g, device=DEV)
+    dh = torch.randn(B, P * D, generator=g, device=DEV)
+    bias = torch.tensor([0.3], device=DEV)
+
+    ops.raw_oob_count()
+    pool = ops.raw_fat_ffm_pool_fwd(W, ids, dense, dense_w, pad, D)
+    assert ops.raw_oob_count() == n_oob
+    y1, h = ops.raw_fat_ffm_fwd(W, ids, dense, dense_w, attn, bias, pad, D)
+    dattn = ops.raw_fat_ffm_bwd_attn(W, ids, dense, dense_w, attn, gy1, dh, pad, D)
+    assert ops.raw_oob_count() == 0
+    assert torch.equal(pool, ops.raw_fat_ffm_pool_fwd(W, ids, dense, dense_w, pad, D)), what + " pool"
+    y1b, hb = ops.raw_fat_ffm_fwd(W, ids, dense, dense_w, attn, bias, pad, D)
+    assert torch.equal(y1, y1b) and torch.equal(h, hb), what + ": fwd not bit-reproducible"
+    del hb
+    assert torch.equal(dattn, ops.raw_fat_ffm_bwd_attn(W, ids, dense, dense_w, attn, gy1, dh, pad, D)), \
+        what + ": dattn not bit-reproducible"
+    ops.raw_oob_count()
+
+    k_y1 = _gamma(_cdiv(NN, 256) * (D + 1) + 14)
+    chunk = _fat_chunk(NF, D)
+    for s in range(0, B, chunk):
+        e = min(B, s + chunk)
+        E = _fat_e(W, ids, dense, dense_w, s, e, D, pad)
+        want_pool, r, m = _fat_closed_form(E, attn[s:e], gy1[s:e], dh[s:e], bias=bias)
+        at = "%s samples %d.." % (what, s)
+        assert torch.equal(pool[s:e], want_pool), at + " pool"
+        assert_within(y1[s:e], r["y1"], k_y1 * m["y1"] + 1e-30, at + " y1")
+        assert_within(h[s:e], r["h"], _gamma(5) * m["h"] + 1e-30, at + " h")
+        assert_within(dattn[s:e], r["dattn"], _gamma(D + 5) * m["dattn"] + 1e-30, at + " dattn")
+
+
+FAT_TIED_ID = 1 + FFM_BWD_LENS.index(150001)
+
+
+def _fat_tied_inputs(W, V, Dn, R, D, NF, B, g):
+    """Quantised inputs full of ties: table and dense_w entries in {-2, -1.75, ..., 2}; every third
+    table row (and ids 1..7) gets one block of nonpositive values holding -0.0 and +0.0 at two
+    different columns; dense values from {-1, -0.5, -0.0, 0, 0.5, 1}."""
+    W[:, :R] = torch.randint(-8, 9, (V, R), generator=g, device=DEV) / 4
+    ar = torch.arange(V, device=DEV)
+    sel = ar[(ar % 3 == 0) | (ar <= len(FFM_BWD_LENS))]
+    m = sel % NF
+    j0 = (sel // NF) % D
+    j1 = (j0 + 1 + (sel // 7) % (D - 1)) % D
+    cols = m.unsqueeze(1) * D + torch.arange(D, device=DEV)
+    W[sel.unsqueeze(1), cols] = -(torch.randint(1, 9, (sel.numel(), D), generator=g, device=DEV) / 4)
+    W[sel, m * D + j0] = -0.0
+    W[sel, m * D + j1] = 0.0
+    dense = torch.tensor([-1, -0.5, -0.0, 0.0, 0.5, 1.0], device=DEV)[
+        torch.randint(0, 6, (B, Dn), generator=g, device=DEV)]
+    dense_w = torch.randint(-8, 9, (Dn, R), generator=g, device=DEV) / 4
+    return dense, dense_w
+
+
+@pytest.mark.parametrize("Dn,D,B,tied", [
+    (13, 10, 65536, False),    # the benchmark shape: 256 full slices
+    (13, 10, 65536 - 100, False),   # a short last slice
+    (13, 10, 65536, True),     # tied block maxima: the first maximum takes the pool gradient
+    (0, 4, 65536, False),      # no dense fields
+    (13, 1, 65536, False),     # every column is its block's maximum
+])
+def test_fat_bwd_at_scale(Dn, D, B, tied):
+    """raw_fat_ffm_bwd (FatBwd on ffm_bwd_light / hot / combine / dense kernels) at B*F = 1.7M
+    positions, F=26, V=200k, with _ffm_bwd_ids' stream: every light warp walks >= 3 distinct ids,
+    every hot CTA takes >= 3 work items, and the combine adds the 147 chunks of the
+    150001-position id.  Every row of every distinct id is checked element-wise against the
+    per-position de of _fat_closed_form merged in fp64 with index_add, bound gamma(ffm_bwd_chain
+    + 4): FFM's chain with 6 roundings per term instead of 2 (the partner product, dh fma, attn
+    product, the dense product, the pool add).  Columns R..G-1 (the w1 column and the padding)
+    must be exactly 0.  Dense gradients over `slices` = min(256, ceil(B/256)) slices of per_slice
+    samples: ddense_w gamma(per_slice + slices + 6), dbias gamma(per_slice + slices).  Every
+    output is bit-identical on a second run.
+    tied: table and dense_w entries are multiples of 1/4 in [-2, 2], some table blocks hold both
+    -0.0 and +0.0 as their maximum, dense values include -0.0 and 0, and the inputs are asserted
+    to hold blocks whose first and last maxima differ for a light id, a single-chunk hot id and
+    the 150001-position id: a last-maximum rule moves dpool to another column of their rows."""
+    ops = _ops()
+    SM = _sm()
+    F, V, pad = 26, 200_000, 0
+    NF = F + Dn
+    R, P, NN = NF * D, NF * (NF - 1) // 2, NF * NF
+    G = ffm_staged_cols(R)
+    n = B * F
+    assert n < FAT_MAX_POSITIONS
+    g = torch.Generator(device=DEV).manual_seed(100 * D + Dn + B + tied)
+    ids = _ffm_bwd_ids(B, F, V, g)
+    flat = ids.reshape(-1)
+    valid = (flat >= 0) & (flat < V) & (flat != pad)
+    uniq, inv, counts = torch.unique(flat[valid], return_inverse=True, return_counts=True)
+    Uq = uniq.numel()
+    assert sorted(counts[counts > 300].tolist()) == sorted(c for c in FFM_BWD_LENS if c > 300)
+    wpb = FFM_THREADS // 32
+    assert int((counts <= HOT_THRESHOLD).sum()) >= 3 * FFM_LIGHT_CTAS_PER_SM * SM * wpb
+    lgrid = min(_cdiv(n, wpb), FFM_LIGHT_CTAS_PER_SM * SM)
+    assert_loops("ffm_bwd_light_kernel<FatBwd>: distinct ids per warp", Uq // (lgrid * wpb))
+    hot = counts[counts > HOT_THRESHOLD]
+    n_items = int(((hot + FFM_HOT_CHUNK - 1) // FFM_HOT_CHUNK).sum())
+    hgrid = min(n // (HOT_THRESHOLD + 1) + 1, FFM_HOT_CTAS_PER_SM * SM)
+    assert_loops("ffm_bwd_hot_kernel<FatBwd>: work items per CTA", n_items // hgrid)
+    assert_loops("ffm_bwd_combine_kernel: chunks of the 150001-position id",
+                 _cdiv(FFM_BWD_LENS[-1], FFM_HOT_CHUNK))
+    slices = min(FFM_MAX_SLICES, _cdiv(B, 256))
+    per_slice = _cdiv(B, slices)
+    assert_loops("ffm_bwd_dense_kernel<FatBwd>: samples per slice", per_slice)
+
+    W = _ffm_table(V, R, g)
+    W[:, R] = 7.0
+    if tied:
+        dense, dense_w = _fat_tied_inputs(W, V, Dn, R, D, NF, B, g)
+        blk = W[uniq, :R].view(Uq, NF, D)
+        hit = (blk == blk.amax(-1, keepdim=True)).to(torch.int8)
+        split = (hit.argmax(-1) != D - 1 - hit.flip(-1).argmax(-1)).any(1)
+        assert bool(split[counts <= HOT_THRESHOLD].any()), "no light id with a tied block"
+        assert bool(split[(counts > HOT_THRESHOLD) & (counts <= FFM_HOT_CHUNK)].any()), \
+            "no single-chunk hot id with a tied block"
+        assert bool(split[uniq == FAT_TIED_ID].all()), "the 150001-position id has no tied block"
+        del blk, hit
+    else:
+        dense = torch.rand(B, Dn, generator=g, device=DEV) * 2 - 0.5
+        dense_w = torch.randn(Dn, R, generator=g, device=DEV) * 0.1
+    attn = torch.relu(torch.randn(B, NN, generator=g, device=DEV) + 0.3)
+    gy1 = torch.randn(B, generator=g, device=DEV)
+    dh = torch.randn(B, P * D, generator=g, device=DEV)
+    dpool = torch.randn(B, NN, generator=g, device=DEV)
+    groups = ops.raw_group_ids(ids, V, pad)
+    assert int(groups.num[0]) == Uq
+    assert torch.equal(groups.unique_ids[:Uq], uniq), "the gradient rows must be exactly the valid ids"
+    args = (W, ids, dense, dense_w, attn, gy1, dh, dpool, groups, pad, D)
+    dW, ddw, db = ops.raw_fat_ffm_bwd(*args)
+    dW2, ddw2, db2 = ops.raw_fat_ffm_bwd(*args)
+    what = "fat bwd Dn=%d D=%d B=%d%s" % (Dn, D, B, " tied" if tied else "")
+    assert torch.equal(dW[:Uq], dW2[:Uq]), what + ": rows not bit-reproducible"
+    assert torch.equal(ddw, ddw2) and torch.equal(db, db2), what + ": dense gradients not bit-reproducible"
+    del dW2
+    assert dW.shape[1] == G and not dW[:Uq, R:].any(), what + ": columns R.. of the rows must be 0"
+
+    f64 = dict(dtype=torch.float64, device=DEV)
+    pos_row = torch.full((n,), -1, dtype=torch.int64, device=DEV)
+    pos_row[valid] = inv
+    want, mag = torch.zeros(Uq, R, **f64), torch.zeros(Uq, R, **f64)
+    wdw, mdw = torch.zeros(Dn, R, **f64), torch.zeros(Dn, R, **f64)
+    chunk = _fat_chunk(NF, D)
+    for s in range(0, B, chunk):
+        e = min(B, s + chunk)
+        b = e - s
+        E = _fat_e(W, ids, dense, dense_w, s, e, D, pad)
+        _, r, m = _fat_closed_form(E, attn[s:e], gy1[s:e], dh[s:e], dpool[s:e])
+        de, dm = r["de"].view(b, NF, R), m["de"].view(b, NF, R)
+        rr = pos_row[s * F:e * F]
+        ok = rr >= 0
+        want.index_add_(0, rr[ok], de[:, :F].reshape(b * F, R)[ok])
+        mag.index_add_(0, rr[ok], dm[:, :F].reshape(b * F, R)[ok])
+        if Dn:
+            x = dense[s:e].double()
+            wdw += torch.einsum("bk,bkr->kr", x, de[:, F:])
+            mdw += torch.einsum("bk,bkr->kr", x.abs(), dm[:, F:])
+    del E, r, m, de, dm
+    k = _gamma(ffm_bwd_chain(counts) + 4).unsqueeze(1)
+    for r0 in range(0, Uq, 32768):
+        sl = slice(r0, min(Uq, r0 + 32768))
+        assert_within(dW[sl, :R], want[sl], k[sl] * mag[sl] + 1e-30, what + " rows %d.." % r0)
+    del want, mag
+    if Dn:
+        assert_within(ddw, wdw, _gamma(per_slice + slices + 6) * mdw + 1e-30, what + " ddense_w")
+    assert_within(db, gy1.double().sum().reshape(1),
+                  _gamma(per_slice + slices) * gy1.double().abs().sum().reshape(1), what + " dbias")
+
+
+def test_fat_bwd_chunk_packing_limit():
+    """FatBwd on the work-item packing of test_ffm_bwd_chunk_packing_limit: items pack
+    chunk | (chunks << 16) into one int32 (ffm.cuh:287), which the launcher bounds by
+    B*F < 32767*1024 (fat_ffm.cuh:370).  F=1, Dn=0, D=1: NF = 1, so P = 0 and dh has no elements.
+    At B*F = 32767*1024 - 1, id 1 takes 32766*1024 + 512 positions (32767 chunks), all with
+    attn = gy1 = dpool = 1: each contributes attn*gy1 + dpool = 2 (with D = 1 every column is its
+    block's maximum).  A full chunk sums to exactly 2048 (8 warps of 128 twos), every partial total
+    of the combine is a multiple of 1024 below 2^26, so fp32 holds each one exactly and id 1's row
+    must be exactly 2*n_a: a dropped or duplicated chunk shows.  The other 511 positions go to
+    distinct ids, each row one attn*gy1 + dpool (gamma(2)).  dbias: gamma(per_slice + slices).  One
+    more position, with every buffer sized for it, is refused with B200REC_ERR_INVALID naming B*F."""
+    import ctypes
+    from paddlerec_b200 import _lib
+    ops = _ops()
+    lib = _lib.load()
+    SM = _sm()
+    n_max = FAT_MAX_POSITIONS                     # the first B*F the launcher refuses
+    n = n_max - 1
+    n_a = (FFM_MAX_CHUNKS - 1) * FFM_HOT_CHUNK + FFM_HOT_CHUNK // 2
+    chunks = _cdiv(n_a, FFM_HOT_CHUNK)
+    assert chunks == FFM_MAX_CHUNKS and chunks << 16 == 2_147_418_112
+    assert 2 * n_a < 1 << 26
+    hgrid = min(n // (HOT_THRESHOLD + 1) + 1, FFM_HOT_CTAS_PER_SM * SM)
+    assert_loops("ffm_bwd_hot_kernel<FatBwd> at the packing limit: work items per CTA", chunks // hgrid)
+    V, A, D = 1024, 1, 1
+    R = D
+    G = ffm_staged_cols(R)
+    g = torch.Generator(device=DEV).manual_seed(32768)
+    ids = torch.full((n_max, 1), 2, dtype=torch.int64, device=DEV)
+    body = torch.cat([torch.full((n_a,), A, dtype=torch.int64, device=DEV),
+                      torch.arange(2, 2 + n - n_a, device=DEV)])
+    ids[:n, 0] = body[torch.randperm(n, generator=g, device=DEV)]
+    del body
+    hot = ids[:, 0] == A
+    attn = torch.where(hot, 1.0, torch.rand(n_max, generator=g, device=DEV)).unsqueeze(1)
+    gy1 = torch.where(hot, 1.0, torch.randn(n_max, generator=g, device=DEV))
+    dpool = torch.where(hot, 1.0, torch.randn(n_max, generator=g, device=DEV)).unsqueeze(1)
+    dh = torch.empty(n_max, 0, device=DEV)
+    W = _ffm_table(V, R, g)
+    W[:, R] = 7.0
+    dense = torch.empty(n_max, 0, device=DEV)
+    dense_w = torch.empty(0, R, device=DEV)
+    groups = ops.raw_group_ids(ids[:n], V, -1)
+    Uq = int(groups.num[0])
+    assert Uq == 1 + n - n_a
+    assert torch.equal(groups.unique_ids[:Uq], torch.arange(1, 1 + Uq, device=DEV))
+    dW, _, db = ops.raw_fat_ffm_bwd(W, ids[:n], dense[:n], dense_w, attn[:n], gy1[:n], dh[:n], dpool[:n],
+                                    groups, -1, D)
+    assert float(dW[0, 0]) == 2.0 * n_a, "row of the 32767-chunk id: %r, want %d" % (float(dW[0, 0]), 2 * n_a)
+    rest = ~hot[:n]
+    at, g1, dp = attn[:n, 0][rest].double(), gy1[:n][rest].double(), dpool[:n, 0][rest].double()
+    want = torch.zeros(V, dtype=torch.float64, device=DEV)
+    mag = torch.zeros(V, dtype=torch.float64, device=DEV)
+    want[ids[:n, 0][rest]] = at * g1 + dp
+    mag[ids[:n, 0][rest]] = (at * g1).abs() + dp.abs()
+    assert_within(dW[1:Uq, 0], want[2:1 + Uq], _gamma(2) * mag[2:1 + Uq] + 1e-30, "single-position rows")
+    assert not dW[:Uq, R:G].any()
+    slices = min(FFM_MAX_SLICES, _cdiv(n, 256))
+    g1 = gy1[:n].double()
+    assert_within(db, g1.sum().reshape(1), _gamma(_cdiv(n, slices) + slices) * g1.abs().sum().reshape(1),
+                  "dbias at the packing limit")
+
+    nbytes = ctypes.c_size_t(0)
+    assert lib.b200rec_fat_ffm_bwd_workspace_bytes(n_max, 1, 0, D, ctypes.byref(nbytes)) == 0
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=DEV)
+    seg = torch.zeros(n_max + 1, dtype=torch.int32, device=DEV)
+    pos = torch.zeros(n_max, dtype=torch.int32, device=DEV)
+    num = torch.tensor([Uq, n_max], dtype=torch.int32, device=DEV)
+    out = torch.zeros(V, G, device=DEV)
+    P = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
+    rc = lib.b200rec_fat_ffm_bwd(P(W), W.stride(0), P(ids), None, None, P(attn), P(gy1), None, P(dpool),
+                                 P(seg), P(pos), P(num), P(out), G, None, P(db), n_max, 1, 0, D, V, -1,
+                                 P(ws), nbytes.value, None)
+    assert rc == -1 and b"B*F" in lib.b200rec_last_error(), (rc, lib.b200rec_last_error())
