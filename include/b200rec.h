@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define B200REC_ABI_VERSION 5
+#define B200REC_ABI_VERSION 6
 
 #define B200REC_OK 0
 #define B200REC_ERR_INVALID (-1)   /* bad argument (shape, alignment, NULL) */
@@ -185,6 +185,23 @@ int b200rec_fat_ffm_bwd(const float* W, int64_t ldw, const int64_t* ids, const f
  * forward (lookup_table_v2), e.g. models/rank/wide_deep/net.py:90, dcn_v2/net.py:95. */
 int b200rec_gather(const float* W, int64_t ldw, const int64_t* ids, float* out, int64_t n, int D,
                    int64_t V, int64_t padding_idx, void* stream);
+/* GateNet embedding gate fused with the gather and the tower-input concat
+ * (models/rank/gatenet/net.py:88-103,110).  W [V,ldw], ids int64 [B,F] (F <= 256), gate_w [F].
+ *   gate_embed_fwd  out [B, ld_out] (ld_out >= F*D + Dn): out[b, f*D + d] = e_d * g with
+ *                   e = W[ids[b,f], :D], g = 1/(1 + expf(-sum_d e_d * gate_w[f])); the dense
+ *                   features dense [B,Dn] follow at column F*D.  Out-of-range ids: zero row, counted.
+ *   gate_embed_bwd  re-gathers the rows; dout is the gradient of out (pitch ld_out).  Writes the
+ *                   per-position table-gradient rows drow [B*F, D] (to be merged with group_ids +
+ *                   segment_reduce; zero for out-of-range ids) and dgate_w [F], summed in a fixed
+ *                   order (no float atomics: bit-identical across runs). */
+int b200rec_gate_embed_fwd(const float* W, int64_t ldw, const int64_t* ids, const float* gate_w,
+                           const float* dense, float* out, int64_t ld_out, int64_t B, int F, int D,
+                           int Dn, int64_t V, void* stream);
+int b200rec_gate_embed_bwd_workspace_bytes(int64_t B, int F, size_t* bytes_host);
+int b200rec_gate_embed_bwd(const float* W, int64_t ldw, const int64_t* ids, const float* gate_w,
+                           const float* dout, int64_t ld_out, float* drow, float* dgate_w,
+                           int64_t B, int F, int D, int64_t V, void* workspace,
+                           size_t workspace_bytes, void* stream);
 /* rows[u,:] = sum_{p in segment u} dOut[p,:]  — the SelectedRows merge of
  * lookup_table_v2_grad.  Deterministic (fixed order inside a segment); ids occurring more than
  * 64 times are reduced by whole CTAs (skew-proof).  row_of_pos (may be NULL) redirects position p to
@@ -346,6 +363,19 @@ int b200rec_tc_cross_fwd(const void* xl_planes, int64_t lda, const void* wt_plan
                          const float* bias, const float* x0, const float* xl, int64_t ld_x,
                          float* u_f32, float* out_f32, int64_t ld_f32, void* out_planes,
                          int64_t ldp, int ones_col, int64_t M, int C, void* stream);
+/* GateNet hidden gate (models/rank/gatenet/net.py:116-118), z = y * tanh(a) with a = y @ G, G [N,N]:
+ *   tc_gate_fwd   a = y @ G on the K-major wgmma GEMM (y planes [M,2*ldy] are both the A operand and
+ *                 the gate's multiplicand; G^T planes [N,2*ldk]); the epilogue writes a_f32 (may be
+ *                 NULL) and z as fp32 (may be NULL) with pitch ld_f32, and/or planes(z) [M,2*ldp]
+ *                 with the optional column of ones.  tanhf is the accurate one.
+ *   tc_gate_bwd   given dz fp32 [M,N] and a fp32 [M,N] (both contiguous): planes(g) [M,2*ldp] with
+ *                 g = dz * y * (1 - tanh(a)^2) and r = dz * tanh(a) fp32 [M,N].  Then
+ *                 dG = tc_linear_bwd_dw(y, g) and dy = tc_linear_bwd_dx(g, G, mask = y, addend = r). */
+int b200rec_tc_gate_fwd(const void* y_planes, int64_t ldy, const void* gt_planes, int64_t ldk,
+                        float* a_f32, float* out_f32, int64_t ld_f32, void* out_planes, int64_t ldp,
+                        int ones_col, int64_t M, int N, void* stream);
+int b200rec_tc_gate_bwd(const float* dz, const void* y_planes, int64_t ldy, const float* a,
+                        void* g_planes, int64_t ldp, float* r, int64_t M, int N, void* stream);
 int b200rec_tc_linear_bwd_workspace_bytes(int64_t M, int K, int N, size_t* bytes_host);
 int b200rec_tc_linear_bwd_dx(const void* g_planes, int64_t ldg, const void* w_planes, int64_t ldn,
                              const void* mask_planes, int64_t ld_mask, const float* addend,

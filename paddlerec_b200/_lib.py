@@ -64,7 +64,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     return LIB_PATH
 
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 _P = c_void_p
 _SIG = {
     "b200rec_abi_version": (c_int, []),
@@ -97,6 +97,11 @@ _SIG = {
                                     _P, _P, c_int64, c_int, c_int, c_int, c_int64, c_int64, _P,
                                     c_size_t, _P]),
     "b200rec_gather": (c_int, [_P, c_int64, _P, _P, c_int64, c_int, c_int64, c_int64, _P]),
+    "b200rec_gate_embed_fwd": (c_int, [_P, c_int64, _P, _P, _P, _P, c_int64, c_int64, c_int, c_int,
+                                       c_int, c_int64, _P]),
+    "b200rec_gate_embed_bwd_workspace_bytes": (c_int, [c_int64, c_int, POINTER(c_size_t)]),
+    "b200rec_gate_embed_bwd": (c_int, [_P, c_int64, _P, _P, _P, c_int64, _P, _P, c_int64, c_int, c_int,
+                                       c_int64, _P, c_size_t, _P]),
     "b200rec_segment_reduce_workspace_bytes": (c_int, [c_int64, c_int, POINTER(c_size_t)]),
     "b200rec_segment_reduce": (c_int, [_P, _P, _P, _P, _P, _P, c_int64, c_int, _P, c_size_t, _P]),
     "b200rec_gather_pool_sum": (c_int, [_P, c_int64, _P, _P, _P, _P, c_int64, c_int, c_int64,
@@ -138,6 +143,9 @@ _SIG = {
                                       c_int, c_int64, c_int, c_int, _P]),
     "b200rec_tc_cross_fwd": (c_int, [_P, c_int64, _P, c_int64, _P, _P, _P, c_int64, _P, _P, c_int64,
                                      _P, c_int64, c_int, c_int64, c_int, _P]),
+    "b200rec_tc_gate_fwd": (c_int, [_P, c_int64, _P, c_int64, _P, _P, c_int64, _P, c_int64, c_int,
+                                    c_int64, c_int, _P]),
+    "b200rec_tc_gate_bwd": (c_int, [_P, _P, c_int64, _P, _P, c_int64, _P, c_int64, c_int, _P]),
     "b200rec_tc_linear_bwd_workspace_bytes": (c_int, [c_int64, c_int, c_int, POINTER(c_size_t)]),
     "b200rec_tc_linear_bwd_dx": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, _P, _P, c_int64, _P,
                                          c_int64, _P, c_int64, c_int, c_int, _P, c_size_t, _P]),

@@ -19,6 +19,7 @@
 #include "din_attn.cuh"
 #include "ffm.cuh"
 #include "fat_ffm.cuh"
+#include "gate_embed.cuh"
 
 namespace b200rec {
 
@@ -252,6 +253,33 @@ int b200rec_gather(const float* W, int64_t ldw, const int64_t* ids, float* out, 
   return launch_gather(W, ids, out, n, D, V, padding_idx, ldw, ST(stream));
 }
 
+int b200rec_gate_embed_fwd(const float* W, int64_t ldw, const int64_t* ids, const float* gate_w,
+                           const float* dense, float* out, int64_t ld_out, int64_t B, int F, int D,
+                           int Dn, int64_t V, void* stream) {
+  if (B > 0) {
+    NOT_NULL(W); NOT_NULL(ids); NOT_NULL(gate_w); NOT_NULL(out);
+    if (Dn > 0) NOT_NULL(dense);
+  }
+  return launch_gate_embed_fwd(W, ldw, ids, gate_w, dense, out, ld_out, B, F, D, Dn, V, ST(stream));
+}
+
+int b200rec_gate_embed_bwd_workspace_bytes(int64_t B, int F, size_t* bytes_host) {
+  NOT_NULL(bytes_host);
+  B200_REQUIRE(B >= 0 && F > 0 && F <= kGateEmbedMaxFields, "gate_embed_bwd_workspace_bytes: bad sizes");
+  *bytes_host = gate_embed_bwd_ws_bytes(B, F) + 16;
+  return B200REC_OK;
+}
+
+int b200rec_gate_embed_bwd(const float* W, int64_t ldw, const int64_t* ids, const float* gate_w,
+                           const float* dout, int64_t ld_out, float* drow, float* dgate_w,
+                           int64_t B, int F, int D, int64_t V, void* workspace,
+                           size_t workspace_bytes, void* stream) {
+  NOT_NULL(dgate_w);
+  if (B > 0) { NOT_NULL(W); NOT_NULL(ids); NOT_NULL(gate_w); NOT_NULL(dout); NOT_NULL(drow); }
+  return launch_gate_embed_bwd(W, ldw, ids, gate_w, dout, ld_out, drow, dgate_w, B, F, D, V,
+                               workspace, workspace_bytes, ST(stream));
+}
+
 int b200rec_segment_reduce_workspace_bytes(int64_t n, int D, size_t* bytes_host) {
   NOT_NULL(bytes_host);
   B200_REQUIRE(n >= 0, "segment_reduce: bad sizes");
@@ -477,6 +505,28 @@ int b200rec_tc_cross_fwd(const void* xl_planes, int64_t lda, const void* wt_plan
   ep.out_f32 = out_f32; ep.ld_f32 = ld_f32;
   ep.out_planes = static_cast<__nv_bfloat16*>(out_planes); ep.ldp = ldp;
   return tc::launch_gemm_kmajor(xl_planes, lda, wt_planes, ldk, M, C, C, ep, ST(stream));
+}
+
+int b200rec_tc_gate_fwd(const void* y_planes, int64_t ldy, const void* gt_planes, int64_t ldk,
+                        float* a_f32, float* out_f32, int64_t ld_f32, void* out_planes, int64_t ldp,
+                        int ones_col, int64_t M, int N, void* stream) {
+  if (M > 0) { NOT_NULL(y_planes); NOT_NULL(gt_planes); }
+  B200_REQUIRE(out_f32 != nullptr || out_planes != nullptr, "tc_gate_fwd: no output");
+  B200_REQUIRE(ldy >= N && ld_f32 >= N, "tc_gate_fwd: ldy or ld_f32 < N");
+  B200_REQUIRE(out_planes == nullptr || ldp >= N + (ones_col ? 1 : 0), "tc_gate_fwd: ldp < N");
+  tc::Epilogue ep = {};
+  ep.ones_col = ones_col;
+  ep.aux_f32 = a_f32; ep.ld_aux = ld_f32;
+  ep.gate_y = static_cast<const __nv_bfloat16*>(y_planes); ep.ld_gate = ldy;
+  ep.out_f32 = out_f32; ep.ld_f32 = ld_f32;
+  ep.out_planes = static_cast<__nv_bfloat16*>(out_planes); ep.ldp = ldp;
+  return tc::launch_gemm_kmajor(y_planes, ldy, gt_planes, ldk, M, N, N, ep, ST(stream));
+}
+
+int b200rec_tc_gate_bwd(const float* dz, const void* y_planes, int64_t ldy, const float* a,
+                        void* g_planes, int64_t ldp, float* r, int64_t M, int N, void* stream) {
+  if (M > 0) { NOT_NULL(dz); NOT_NULL(y_planes); NOT_NULL(a); NOT_NULL(g_planes); NOT_NULL(r); }
+  return launch_tower_gate_bwd(dz, y_planes, ldy, a, g_planes, ldp, r, M, N, ST(stream));
 }
 
 int b200rec_tc_linear_bwd_workspace_bytes(int64_t M, int K, int N, size_t* bytes_host) {

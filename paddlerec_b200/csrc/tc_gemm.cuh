@@ -311,6 +311,11 @@ struct Epilogue {
   int64_t ld_add;
   float* aux_f32;                   // [M, ld_aux] receives acc + bias + addend, i.e. the value BEFORE
   int64_t ld_aux;                   //   the CrossNet / ReLU / mask transforms, or null
+  // GateNet hidden gate (gatenet/net.py:116-118): v = y[m,n] * tanhf(acc), y = hi + lo of the planes
+  // [M, 2*ld_gate] at gate_y (the GEMM's own A operand).  Read only by the kernels compiled with
+  // kGate, so the other instantiations keep their code.
+  const __nv_bfloat16* gate_y;
+  int64_t ld_gate;
   // filled in by launch_gemm_kmajor, not by the callers:
   int vec;                          // kVec* bits: the operand allows one 16-byte (fp32) or 8-byte
                                     //   (bf16) access per 4 columns at every row
@@ -319,7 +324,7 @@ struct Epilogue {
 
 enum : int {
   kVecBias = 1, kVecF32 = 2, kVecPlanes = 4, kVecMask = 8, kVecAdd = 16, kVecAux = 32,
-  kVecCross = 64,
+  kVecCross = 64, kVecGate = 128,
 };
 
 __device__ __forceinline__ void split_bf16(float x, float& hi_f, __nv_bfloat16& hi,
@@ -437,9 +442,10 @@ __device__ __forceinline__ void stage_chunk(const float (&acc)[BN / 2], float* s
 // inputs of the chunk are loaded first, then stage() puts the raw accumulators into `stg`.  The
 // transforms apply in this order: + bias, + addend, aux store, CrossNet fma, ReLU, mask, then the
 // fp32 and hi/lo stores, the same per-element arithmetic as an unstaged epilogue.  kExtra: the
-// addend / aux / CrossNet body; without it those fields are ignored.  With s_cs (the warp's column
-// sums of this chunk) the emitted values are summed over the warp's rows in a fixed order.
-template <bool kExtra, typename Stage>
+// addend / aux / CrossNet body; without it those fields are ignored.  kGate (with kExtra): the hidden
+// gate v = y * tanhf(v) right after the aux store.  With s_cs (the warp's column sums of this chunk)
+// the emitted values are summed over the warp's rows in a fixed order.
+template <bool kExtra, typename Stage, bool kGate = false>
 __device__ __forceinline__ void epilogue_rows(const Epilogue& ep, const float* stg, int M, int N,
                                               int64_t r0, int c0, int cw, int lane, float* s_cs,
                                               Stage stage) {
@@ -485,6 +491,15 @@ __device__ __forceinline__ void epilogue_rows(const Epilogue& ep, const float* s
         v.x = fmaf(x0.x, v.x, xl.x); v.y = fmaf(x0.y, v.y, xl.y);
         v.z = fmaf(x0.z, v.z, xl.z); v.w = fmaf(x0.w, v.w, xl.w);
       }
+      if (kGate) {
+        // accurate tanhf (tanh.approx's ~2^-11 relative error would show in the logit)
+        const __nv_bfloat16* yp = ep.gate_y + row * 2 * ep.ld_gate + col;
+        const uint2 h = ld4_bf16(yp, n, vec & kVecGate), l = ld4_bf16(yp + ep.ld_gate, n, vec & kVecGate);
+        v.x = (__uint_as_float(h.x << 16) + __uint_as_float(l.x << 16)) * tanhf(v.x);
+        v.y = (__uint_as_float(h.x & 0xFFFF0000u) + __uint_as_float(l.x & 0xFFFF0000u)) * tanhf(v.y);
+        v.z = (__uint_as_float(h.y << 16) + __uint_as_float(l.y << 16)) * tanhf(v.z);
+        v.w = (__uint_as_float(h.y & 0xFFFF0000u) + __uint_as_float(l.y & 0xFFFF0000u)) * tanhf(v.w);
+      }
     }
     if (ep.relu) {
       v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
@@ -527,7 +542,7 @@ __device__ __forceinline__ void epilogue_rows(const Epilogue& ep, const float* s
 // One consumer warp's 16 x BN share of a 128 x BN accumulator tile -> outputs, in chunks of 32
 // columns.  r0: the warp's first matrix row.  With s_cs ([kMaxBN]) the warp's column sums of the
 // emitted values land there.  The chunk loop is not unrolled: one copy of each epilogue body.
-template <int BN>
+template <int BN, bool kGate = false>
 __device__ __forceinline__ void epilogue_tile(const Epilogue& ep, const float (&acc)[BN / 2],
                                               float* stg, int M, int N, int64_t r0, int n0, int lane,
                                               float* s_colsum) {
@@ -537,7 +552,10 @@ __device__ __forceinline__ void epilogue_tile(const Epilogue& ep, const float (&
     const int cw = BN - kEpCols * c < kEpCols ? BN - kEpCols * c : kEpCols;
     float* s_cs = s_colsum != nullptr ? s_colsum + kEpCols * c : nullptr;
     auto stage = [&] { stage_chunk<BN>(acc, stg, c, lane); };
-    if (ep.extra)
+    if constexpr (kGate)
+      epilogue_rows<true, decltype(stage), true>(ep, stg, M, N, r0, n0 + kEpCols * c, cw, lane, s_cs,
+                                                 stage);
+    else if (ep.extra)
       epilogue_rows<true>(ep, stg, M, N, r0, n0 + kEpCols * c, cw, lane, s_cs, stage);
     else
       epilogue_rows<false>(ep, stg, M, N, r0, n0 + kEpCols * c, cw, lane, s_cs, stage);
@@ -566,15 +584,27 @@ __device__ __forceinline__ void epilogue_prefetch(const Epilogue& ep, int M, int
   }
 }
 
+// The gate's y planes (hi and lo) of a warp's 16 rows, fetched like the side inputs above.
+__device__ __forceinline__ void epilogue_prefetch_gate(const Epilogue& ep, int M, int N, int BN,
+                                                      int64_t r0, int n0, int lane) {
+  const int64_t row = r0 + (lane >> 1);
+  if (row >= M) return;
+  const int w = N - n0 < BN ? N - n0 : BN;
+  const __nv_bfloat16* y = ep.gate_y + row * 2 * ep.ld_gate + n0;
+  prefetch_row_l2(y, 2 * w, lane);
+  prefetch_row_l2(y + ep.ld_gate, 2 * w, lane);
+}
+
 // ------------------------------------------------------------------------------------------------
 // K-major GEMM: D[M,N] = A[M,K] . B[N,K]^T  (three wgmma per 16-wide k step)
 //   BK = 64: 128-byte swizzle rows (2 pipeline stages at BN = 208)
 //   BK = 32: 64-byte swizzle rows, half-size stages -> 4 stages at BN = 208: about the same bytes in
 //            shared memory, but a freed slot is refilled twice as early, which hides the TMA latency
 // The producer warpgroup hands registers to the consumers (setmaxnreg): a consumer thread holds
-// BN / 2 accumulators through the whole epilogue.
+// BN / 2 accumulators through the whole epilogue.  kGate: the GateNet hidden-gate epilogue
+// (Epilogue::gate_y), a separate instantiation so the plain and CrossNet kernels stay as they are.
 // ------------------------------------------------------------------------------------------------
-template <int BN, int BK>
+template <int BN, int BK, bool kGate = false>
 __global__ void __launch_bounds__(kThreads, 1)
 tc_gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA_hi,
                       const __grid_constant__ CUtensorMap tmA_lo,
@@ -651,6 +681,7 @@ tc_gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA_hi,
       const int m0 = m_blk * kBM, n0 = (tile % tiles_n) * BN;
       const int64_t r0 = (int64_t)m0 + 64 * wg + 16 * (cw & 3);   // this warp's first row
       epilogue_prefetch(ep, M, N, BN, r0, n0, lane);
+      if constexpr (kGate) epilogue_prefetch_gate(ep, M, N, BN, r0, n0, lane);
       int prev = 0;
       // one k-block of NS 16-wide k-steps: three wgmma per step, one commit group per block
       auto kblock = [&](auto ns, int kb) {
@@ -690,7 +721,7 @@ tc_gemm_kmajor_kernel(const __grid_constant__ CUtensorMap tmA_hi,
       wgmma_wait<0>();
       fence_acc(acc);
       if (lane == 0) mbar_arrive(bar_empty + 8u * prev);
-      epilogue_tile<BN>(ep, acc, stg, M, N, r0, n0, lane,
+      epilogue_tile<BN, kGate>(ep, acc, stg, M, N, r0, n0, lane,
                         want_colsum ? s_colsum + cw * kMaxBN : nullptr);
       if (want_colsum) {
         named_bar_sync(1, 32 * kConsumerWarps);
@@ -983,7 +1014,7 @@ static int pick_bn(int N) {
   return best;
 }
 
-template <int BN, int BK>
+template <int BN, int BK, bool kGate>
 static int launch_kmajor_tiles(const CUtensorMap (&mp)[4], int64_t M, int N, int K,
                                const Epilogue& ep, cudaStream_t st) {
   constexpr uint32_t stage_bytes = (2u * kBM + 2u * BN) * (uint32_t)BK * 2u;
@@ -995,27 +1026,27 @@ static int launch_kmajor_tiles(const CUtensorMap (&mp)[4], int64_t M, int N, int
   const size_t smem = (size_t)stages * stage_bytes + 16 * stages + scratch + 1024;
   static bool attr_set = false;
   if (!attr_set) {
-    B200_CUDA(cudaFuncSetAttribute(tc_gemm_kmajor_kernel<BN, BK>,
+    B200_CUDA(cudaFuncSetAttribute(tc_gemm_kmajor_kernel<BN, BK, kGate>,
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
   const int tiles = (int)((M + kBM - 1) / kBM) * ((N + BN - 1) / BN);
   const int grid = tiles < sm_count() ? tiles : sm_count();
-  tc_gemm_kmajor_kernel<BN, BK><<<grid, kThreads, smem, st>>>(mp[0], mp[1], mp[2], mp[3], (int)M, N,
-                                                              K, stages, ep);
+  tc_gemm_kmajor_kernel<BN, BK, kGate><<<grid, kThreads, smem, st>>>(mp[0], mp[1], mp[2], mp[3],
+                                                                     (int)M, N, K, stages, ep);
   B200_LAUNCH_CHECK();
   return B200REC_OK;
 }
 
-template <int BK>
+template <int BK, bool kGate>
 static int launch_kmajor_bk(int BN, const CUtensorMap (&mp)[4], int64_t M, int N, int K,
                             const Epilogue& ep, cudaStream_t st) {
   switch (BN) {
-    case 16: return launch_kmajor_tiles<16, BK>(mp, M, N, K, ep, st);
-    case 64: return launch_kmajor_tiles<64, BK>(mp, M, N, K, ep, st);
-    case 128: return launch_kmajor_tiles<128, BK>(mp, M, N, K, ep, st);
-    case 208: return launch_kmajor_tiles<208, BK>(mp, M, N, K, ep, st);
-    default: return launch_kmajor_tiles<256, BK>(mp, M, N, K, ep, st);
+    case 16: return launch_kmajor_tiles<16, BK, kGate>(mp, M, N, K, ep, st);
+    case 64: return launch_kmajor_tiles<64, BK, kGate>(mp, M, N, K, ep, st);
+    case 128: return launch_kmajor_tiles<128, BK, kGate>(mp, M, N, K, ep, st);
+    case 208: return launch_kmajor_tiles<208, BK, kGate>(mp, M, N, K, ep, st);
+    default: return launch_kmajor_tiles<256, BK, kGate>(mp, M, N, K, ep, st);
   }
 }
 
@@ -1038,8 +1069,11 @@ static int launch_gemm_kmajor(const void* A, int64_t lda, const void* B, int64_t
            (aligned_rows(ep.addend, ep.ld_add, 16) ? kVecAdd : 0) |
            (aligned_rows(ep.aux_f32, ep.ld_aux, 16) ? kVecAux : 0) |
            (aligned_rows(ep.cross_x0, ep.ld_cross, 16) && aligned_rows(ep.cross_xl, ep.ld_cross, 16)
-                ? kVecCross : 0);
-  ep.extra = ep.addend != nullptr || ep.aux_f32 != nullptr || ep.cross_x0 != nullptr;
+                ? kVecCross : 0) |
+           (aligned_rows(ep.gate_y, ep.ld_gate, 8) ? kVecGate : 0);
+  ep.extra = ep.addend != nullptr || ep.aux_f32 != nullptr || ep.cross_x0 != nullptr ||
+             ep.gate_y != nullptr;
+  const bool gate = ep.gate_y != nullptr;
   const int BN = pick_bn(N);
   const int BK = g_bk;
   const __nv_bfloat16* a = static_cast<const __nv_bfloat16*>(A);
@@ -1050,8 +1084,11 @@ static int launch_gemm_kmajor(const void* A, int64_t lda, const void* B, int64_t
   if ((rc = make_map(&mp[1], a + lda, K, M, 2 * lda, BK, kBM)) != B200REC_OK) return rc;
   if ((rc = make_map(&mp[2], b, K, N, 2 * ldb, BK, BN)) != B200REC_OK) return rc;
   if ((rc = make_map(&mp[3], b + ldb, K, N, 2 * ldb, BK, BN)) != B200REC_OK) return rc;
-  return BK == 64 ? launch_kmajor_bk<64>(BN, mp, M, N, K, ep, st)
-                  : launch_kmajor_bk<32>(BN, mp, M, N, K, ep, st);
+  if (gate)
+    return BK == 64 ? launch_kmajor_bk<64, true>(BN, mp, M, N, K, ep, st)
+                    : launch_kmajor_bk<32, true>(BN, mp, M, N, K, ep, st);
+  return BK == 64 ? launch_kmajor_bk<64, false>(BN, mp, M, N, K, ep, st)
+                  : launch_kmajor_bk<32, false>(BN, mp, M, N, K, ep, st);
 }
 
 struct DwPlan {

@@ -152,6 +152,47 @@ tower_relu_bwd_split_kernel(const float* __restrict__ dy, const __nv_bfloat16* _
   }
 }
 
+// Backward of the GateNet hidden gate z = y * tanh(a), a = y @ G (gatenet/net.py:116-118), given dz:
+//   planes(g) with g = dz * y * (1 - tanh(a)^2)   (the operand of dG = y^T g and of g @ G^T)
+//   r = dz * tanh(a)                               (fp32, the addend of that dX GEMM)
+// y = hi + lo of its planes, exactly the value the forward epilogue multiplied.  One streaming pass.
+template <int VEC>
+__global__ void __launch_bounds__(kTowerThreads)
+tower_gate_bwd_kernel(const float* __restrict__ dz, const __nv_bfloat16* __restrict__ y, int64_t ldy,
+                      const float* __restrict__ a, __nv_bfloat16* __restrict__ g, int64_t ldp,
+                      float* __restrict__ r, int64_t M, int N) {
+  const int chunks = N / VEC;
+  const int64_t total = M * chunks;
+  for (int64_t i = (int64_t)blockIdx.x * kTowerThreads + threadIdx.x; i < total;
+       i += (int64_t)gridDim.x * kTowerThreads) {
+    const int64_t m = i / chunks;
+    const int c = (int)(i - m * chunks) * VEC;
+    const Vec<VEC> d = ld_row<VEC>(dz + (size_t)m * N + c);
+    const Vec<VEC> t = ld_row<VEC>(a + (size_t)m * N + c);
+    const __nv_bfloat16* yr = y + (size_t)m * 2 * ldy + c;
+    Vec<VEC> gv, rv;
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) {
+      const float yv = __bfloat162float(yr[j]) + __bfloat162float(yr[ldy + j]);
+      const float th = tanhf(t.v[j]);
+      gv.v[j] = d.v[j] * yv * (1.f - th * th);
+      rv.v[j] = d.v[j] * th;
+    }
+    st_plain<VEC>(r + (size_t)m * N + c, rv);
+    __nv_bfloat16* row = g + (size_t)m * 2 * ldp;
+    if (VEC == 4) {
+      Bf16x4 hi, lo;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) split1(gv.v[j], hi.v[j], lo.v[j]);
+      *reinterpret_cast<Bf16x4*>(row + c) = hi;
+      *reinterpret_cast<Bf16x4*>(row + ldp + c) = lo;
+    } else {
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) split1(gv.v[j], row[c + j], row[ldp + c + j]);
+    }
+  }
+}
+
 // W fp32 [K,N] -> W2r bf16 [2K,N] = [hi; hi],  W2c bf16 [K,2N] = [hi | hi],  Wlo bf16 [K,N]
 __global__ void tower_prep_weight_kernel(const float* __restrict__ W,
                                          __nv_bfloat16* __restrict__ W2r,
@@ -394,6 +435,25 @@ static int launch_tower_relu_bwd_split(const float* dy, const void* act, int64_t
   B200_LAUNCH_CHECK();
   reduce_partials_kernel<<<reduce_partials_grid(N), kRedThreads, 0, st>>>(partials, slices, N, dbias, N,
                                                                           nullptr);
+  B200_LAUNCH_CHECK();
+  return B200REC_OK;
+}
+
+static int launch_tower_gate_bwd(const float* dz, const void* y, int64_t ldy, const float* a,
+                                 void* g, int64_t ldp, float* r, int64_t M, int N, cudaStream_t st) {
+  B200_REQUIRE(N > 0 && M >= 0 && ldy >= N && ldp >= N, "tc_gate_bwd: bad sizes");
+  if (M == 0) return B200REC_OK;
+  const bool v4 = (N % 4 == 0) && (ldy % 4 == 0) && (ldp % 4 == 0) && aligned16(dz) &&
+                  aligned16(a) && aligned16(r) && aligned8(y) && aligned8(g);
+  const int64_t total = M * (v4 ? N / 4 : N);
+  const unsigned grid =
+      (unsigned)min((total + kTowerThreads - 1) / kTowerThreads, (int64_t)sm_count() * 16);
+  const __nv_bfloat16* yp = static_cast<const __nv_bfloat16*>(y);
+  __nv_bfloat16* gp = static_cast<__nv_bfloat16*>(g);
+  if (v4)
+    tower_gate_bwd_kernel<4><<<grid, kTowerThreads, 0, st>>>(dz, yp, ldy, a, gp, ldp, r, M, N);
+  else
+    tower_gate_bwd_kernel<1><<<grid, kTowerThreads, 0, st>>>(dz, yp, ldy, a, gp, ldp, r, M, N);
   B200_LAUNCH_CHECK();
   return B200REC_OK;
 }

@@ -49,6 +49,7 @@ KERNELS_PER_CALL = {
     "tc_prep_weight": 1, "tc_linear_fwd": 1, "tc_cross_fwd": 1, "tc_linear_bwd_dx": 1,
     "tc_linear_bwd_dx_db": 2, "tc_linear_bwd_dw": 2, "tc_head_fwd": 1, "tc_head_bwd": 2,
     "auc_update": 1, "sum_sigmoid_fwd": 1, "sum_sigmoid_bwd": 1, "log_loss_mean_fwd": 1, "log_loss_mean_bwd": 1, "din_attn_fwd": 2, "din_attn_bwd": 3, "gather_pool_sum": 2, "cvm_fwd": 1, "cvm_bwd": 1, "hash_keys": 1, "dot_interact_fwd": 1, "dot_interact_bwd": 1,
+    "gate_embed_fwd": 1, "gate_embed_bwd": 2, "tc_gate_fwd": 1, "tc_gate_bwd": 1,
 }
 # When set to a list, (name, start_event, end_event) triples are appended around the raw_* calls
 # (all of them, or only the names in EVENT_FILTER when that is a set) — bench.py's per-kernel times.
@@ -456,6 +457,51 @@ def raw_gather(W: torch.Tensor, ids: torch.Tensor, padding_idx: int,
     return out
 
 
+def raw_gate_embed_fwd(W: torch.Tensor, ids: torch.Tensor, gate_w: torch.Tensor,
+                       dense: Optional[torch.Tensor], D: Optional[int] = None) -> torch.Tensor:
+    """GateNet's gated lookup and tower input (gatenet/net.py:88-110): out [B, F*D + Dn] with
+    out[b, f*D:(f+1)*D] = e * sigmoid(sum(e * gate_w[f])), e = W[ids[b,f], :D], then dense [B,Dn]."""
+    lib = _lib.load()
+    W = _req(W, torch.float32, "W")
+    ids = _req(ids, torch.int64, "ids")
+    gate_w = _req(gate_w.detach().reshape(-1), torch.float32, "gate_w")
+    V, ldw = W.shape
+    D = ldw if D is None else D
+    B, F = ids.shape
+    Dn = 0 if dense is None else dense.shape[1]
+    if dense is not None:
+        dense = _req(dense, torch.float32, "dense")
+    out = torch.empty(B, F * D + Dn, dtype=torch.float32, device=W.device)
+    check(lib.b200rec_gate_embed_fwd(ptr(W), ldw, ptr(ids), ptr(gate_w), ptr(dense), ptr(out),
+                                     out.shape[1], B, F, D, Dn, V, _stream()), "gate_embed_fwd")
+    _count("gate_embed_fwd")
+    return out
+
+
+def raw_gate_embed_bwd(W: torch.Tensor, ids: torch.Tensor, gate_w: torch.Tensor, dout: torch.Tensor,
+                       D: Optional[int] = None):
+    """Backward of raw_gate_embed_fwd from dout [B, >= F*D] (the dense columns are ignored):
+    (per-position table-gradient rows [B*F, D], dgate_w [F])."""
+    lib = _lib.load()
+    W = _req(W, torch.float32, "W")
+    ids = _req(ids, torch.int64, "ids")
+    gate_w = _req(gate_w.detach().reshape(-1), torch.float32, "gate_w")
+    dout = _req(dout, torch.float32, "dout")
+    V, ldw = W.shape
+    D = ldw if D is None else D
+    B, F = ids.shape
+    drow = torch.empty(B * F, D, dtype=torch.float32, device=W.device)
+    dgate = torch.empty(F, dtype=torch.float32, device=W.device)
+    nbytes = ctypes.c_size_t(0)
+    check(lib.b200rec_gate_embed_bwd_workspace_bytes(B, F, ctypes.byref(nbytes)), "gate_embed_bwd_ws")
+    ws = workspace(nbytes.value, W.device, "gate_embed")
+    check(lib.b200rec_gate_embed_bwd(ptr(W), ldw, ptr(ids), ptr(gate_w), ptr(dout), dout.shape[1],
+                                     ptr(drow), ptr(dgate), B, F, D, V, ptr(ws), ws.numel(),
+                                     _stream()), "gate_embed_bwd")
+    _count("gate_embed_bwd")
+    return drow, dgate
+
+
 def raw_gather_pool_sum(W, keys, offsets, padding_idx: int, D: Optional[int] = None):
     """Sum-pooled lookup of variable-length key lists.  keys int64 [nnz], offsets int64
     [n_bags+1].  Returns (out [n_bags, D], bag_of_pos int32 [nnz])."""
@@ -782,6 +828,38 @@ def raw_tc_cross_fwd(xl_planes, WTp, bias, x0, xl, want_planes: bool, want_u: bo
                                    int(ones_col and want_planes), M, C, _stream()), "tc_cross_fwd")
     _count("tc_cross_fwd")
     return out, op, u
+
+
+def raw_tc_gate_fwd(y_planes, GTp, N: int, want_a: bool, want_f32: bool, want_planes: bool,
+                    ones_col: bool = False):
+    """GateNet hidden gate z = y * tanh(a), a = y @ G, on the wgmma GEMM with the gate in the
+    epilogue (y planes [M, 2*ld], GTp = planes(G^T)).  Returns (z fp32 | None, planes(z) | None,
+    a fp32 | None)."""
+    lib = _lib.load()
+    M = y_planes.shape[0]
+    dev = y_planes.device
+    z = torch.empty(M, N, dtype=torch.float32, device=dev) if want_f32 else None
+    a = torch.empty(M, N, dtype=torch.float32, device=dev) if want_a else None
+    zp = _planes(M, N, dev, ones_col) if want_planes else None
+    check(lib.b200rec_tc_gate_fwd(ptr(y_planes), y_planes.shape[1] // 2, ptr(GTp), GTp.shape[1] // 2,
+                                  ptr(a), ptr(z), N, ptr(zp), zp.shape[1] // 2 if zp is not None else 0,
+                                  int(ones_col and want_planes), M, N, _stream()), "tc_gate_fwd")
+    _count("tc_gate_fwd")
+    return z, zp, a
+
+
+def raw_tc_gate_bwd(dz: torch.Tensor, y_planes, a: torch.Tensor):
+    """Backward of the hidden gate: (planes(dz * y * (1 - tanh(a)^2)), dz * tanh(a) fp32)."""
+    lib = _lib.load()
+    dz = _req(dz, torch.float32, "dz")
+    a = _req(a, torch.float32, "a")
+    M, N = dz.shape
+    g = _planes(M, N, dz.device)
+    r = torch.empty(M, N, dtype=torch.float32, device=dz.device)
+    check(lib.b200rec_tc_gate_bwd(ptr(dz), ptr(y_planes), y_planes.shape[1] // 2, ptr(a), ptr(g),
+                                  g.shape[1] // 2, ptr(r), M, N, _stream()), "tc_gate_bwd")
+    _count("tc_gate_bwd")
+    return g, r
 
 
 def _tc_bwd_ws(M: int, K: int, N: int, device, tag: str = "tc_bwd") -> torch.Tensor:
@@ -1211,6 +1289,34 @@ class _GatherPool(torch.autograd.Function):
                                   groups.num, groups.n, row_of_pos=bag_of_pos)
         ctx.sink.accept(SelectedRows(groups.unique_ids, rows, groups.num, ctx.V))
         return None, None, None, None, None, None
+
+
+class _GateEmbed(torch.autograd.Function):
+    """GateNet's embedding gate, gathered lookup and tower-input concat (gatenet/net.py:88-110) in one
+    kernel each way.  The table gradient goes to `sink` as one SelectedRows (grouped and merged as
+    _Gather.backward does); the [F] gate-weight gradient is returned."""
+
+    @staticmethod
+    def forward(ctx, gate_w, W, ids, dense, sink, D):
+        out = raw_gate_embed_fwd(W, ids, gate_w, dense, D)
+        ctx.save_for_backward(W, ids, gate_w)
+        ctx.sink, ctx.D = sink, D
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        W, ids, gate_w = ctx.saved_tensors
+        drow, dgate = raw_gate_embed_bwd(W, ids, gate_w, dout.contiguous(), ctx.D)
+        V = W.shape[0]
+        groups = raw_group_ids(ids, V, -1)
+        rows = raw_segment_reduce(drow, groups.seg_offsets, groups.sorted_pos, groups.num, groups.n)
+        ctx.sink.accept(SelectedRows(groups.unique_ids, rows, groups.num, V))
+        return dgate.reshape(gate_w.shape), None, None, None, None, None
+
+
+def gate_embed(gate_w, W, ids, dense, sink, D=None):
+    """[B, F*D + Dn] gated tower input; gate_w [F] carries the autograd edge."""
+    return _GateEmbed.apply(gate_w, W, ids, dense, sink, D)
 
 
 def gather_pool_sum(W, keys, offsets, padding_idx, sink, hook):
@@ -1705,6 +1811,7 @@ for _n in ("group_ids", "embed_fm_bwd", "ffm_fwd", "ffm_bwd", "fat_ffm_pool_fwd"
            "shard_gather_push", "shard_push_rows", "shard_fm_grads_push",
            "tc_split", "tc_split_bwd", "tc_prep_weight", "tc_linear_fwd", "tc_cross_fwd",
            "tc_linear_bwd_dx", "tc_linear_bwd_dw", "tc_head_fwd", "tc_head_bwd", "din_attn_fwd", "din_attn_bwd", "tower_split",
-           "tower_relu_bwd_split", "tower_prep_weight", "tower_fold_dw"):
+           "tower_relu_bwd_split", "tower_prep_weight", "tower_fold_dw", "gate_embed_fwd",
+           "gate_embed_bwd", "tc_gate_fwd", "tc_gate_bwd"):
     globals()["raw_" + _n] = _wrap_timed(globals()["raw_" + _n], _n)
 del _n

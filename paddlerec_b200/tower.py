@@ -25,7 +25,7 @@ Two back ends with the same arithmetic (three bf16 products per fp32 product, fp
 from __future__ import annotations
 
 import os
-from typing import List, Sequence
+from typing import List, Optional, Sequence
 
 import torch
 
@@ -179,6 +179,88 @@ class _TowerTcFn(torch.autograd.Function):
         return (dx0, None, None, *dWs, *dbs)
 
 
+class _GatedTowerTcFn(torch.autograd.Function):
+    """GateNet's tower (gatenet/net.py:112-119) on the wgmma kernels: every hidden layer is
+    y = relu(x @ W + b) followed by the hidden gate z = y * tanh(y @ G), the last layer is a plain
+    Linear.  The gate GEMM reads planes(y), which the Linear's epilogue emitted, and applies the gate
+    in its own epilogue (b200rec_tc_gate_fwd).  Saved for backward: planes of every layer input,
+    planes(y), a = y @ G (fp32), planes(W) and planes(G).
+
+    z can be negative, so no layer input here is a ReLU output: the dX GEMM that produces dz runs
+    without a mask, and a width-1 last layer takes the generic GEMMs (tc_head_bwd always masks).
+    Per hidden layer, from dz:  (g, r) = tc_gate_bwd(dz, y, a);  dG = y^T g;
+    du = mask_{y>0}(g @ G^T + r) (with db = colsum(du) in the same epilogue);  dW = x^T du;
+    dz_prev = du @ W^T.  The dW GEMMs stay on the current stream."""
+
+    @staticmethod
+    def forward(ctx, x, n_layers, *params):
+        Ws, bs, Gs = params[:n_layers], params[n_layers:2 * n_layers], params[2 * n_layers:]
+        ones = [b is not None and W.shape[0] % 128 != 0 for W, b in zip(Ws, bs)]
+        keep = any(ctx.needs_input_grad)
+        xs = [ops.raw_tc_split(x, ones_col=ones[0])]
+        ys, gate_a, wps, gps = [], [], [], []
+        out = None
+        for i in range(n_layers):
+            K, N = Ws[i].shape
+            Wp, WTp = ops.raw_tc_prep_weight(Ws[i], want_w=keep)
+            wps.append(Wp)
+            if i == n_layers - 1:
+                out, _ = ops.raw_tc_linear_fwd(xs[i], K, WTp, N, bs[i], False, want_f32=True,
+                                               want_planes=False)
+                break
+            _, y = ops.raw_tc_linear_fwd(xs[i], K, WTp, N, bs[i], True, want_f32=False,
+                                         want_planes=True)
+            Gp, GTp = ops.raw_tc_prep_weight(Gs[i], want_w=keep)
+            _, z, a = ops.raw_tc_gate_fwd(y, GTp, N, want_a=keep, want_f32=False, want_planes=True,
+                                          ones_col=ones[i + 1])
+            ys.append(y)
+            gate_a.append(a)
+            gps.append(Gp)
+            xs.append(z)
+        ctx.n_layers, ctx.ones = n_layers, ones
+        ctx.xs, ctx.ys, ctx.gate_a, ctx.wps, ctx.gps = xs, ys, gate_a, wps, gps
+        ctx.shapes = [tuple(W.shape) for W in Ws]
+        ctx.has_bias = [b is not None for b in bs]
+        return out
+
+    @staticmethod
+    def backward(ctx, dy):
+        n, ones, shapes = ctx.n_layers, ctx.ones, ctx.shapes
+        xs, ys, gate_a, wps, gps = ctx.xs, ctx.ys, ctx.gate_a, ctx.wps, ctx.gps
+        dWs, dbs, dGs = [None] * n, [None] * n, [None] * (n - 1)
+
+        def linear_dw(i, g, db_epilogue):
+            K, N = shapes[i]
+            if ones[i]:
+                dWs[i], dbs[i] = ops.raw_tc_linear_bwd_dw(xs[i], K, g, N, bias_row=True)
+            else:
+                dWs[i] = ops.raw_tc_linear_bwd_dw(xs[i], K, g, N)
+                dbs[i] = db_epilogue if ctx.has_bias[i] else None
+
+        top = n - 1
+        K, N = shapes[top]
+        g, db = ops.raw_tc_split_bwd(dy.contiguous(), None)        # no mask: z is not a ReLU output
+        linear_dw(top, g, db)
+        dx0 = None
+        if top > 0 or ctx.needs_input_grad[0]:
+            dx0, _, _ = ops.raw_tc_linear_bwd_dx(g, N, wps[top], K, None, want_f32=True,
+                                                 want_planes=False, want_dbias=False)
+        for i in range(n - 2, -1, -1):
+            K, N = shapes[i]
+            dz, dx0 = dx0, None
+            ga, r = ops.raw_tc_gate_bwd(dz, ys[i], gate_a[i])
+            dGs[i] = ops.raw_tc_linear_bwd_dw(ys[i], N, ga, N)
+            want_db = ctx.has_bias[i] and not ones[i]
+            _, du, db = ops.raw_tc_linear_bwd_dx(ga, N, gps[i], N, ys[i], want_f32=False,
+                                                 want_planes=True, want_dbias=want_db, addend=r)
+            linear_dw(i, du, db)
+            if i > 0 or ctx.needs_input_grad[0]:
+                dx0, _, _ = ops.raw_tc_linear_bwd_dx(du, N, wps[i], K, None, want_f32=True,
+                                                     want_planes=False, want_dbias=False)
+        ctx.xs = ctx.ys = ctx.gate_a = ctx.wps = ctx.gps = None
+        return (dx0 if ctx.needs_input_grad[0] else None, None, *dWs, *dbs, *dGs)
+
+
 class _TowerFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, n_layers, last_act, *params):
@@ -236,9 +318,21 @@ class _TowerFn(torch.autograd.Function):
 
 
 def mlp(x: torch.Tensor, weights: Sequence[torch.Tensor], biases: Sequence[torch.Tensor],
-        last_act: bool = False) -> torch.Tensor:
-    """relu(...relu(x@W0+b0)...)@W_last+b_last  (ReLU after the last layer iff last_act)."""
+        last_act: bool = False, gates: Optional[Sequence[torch.Tensor]] = None) -> torch.Tensor:
+    """relu(...relu(x@W0+b0)...)@W_last+b_last  (ReLU after the last layer iff last_act).
+
+    With `gates` (one [N_i, N_i] matrix per hidden layer) every hidden layer is followed by
+    GateNet's hidden gate y * tanh(y @ G_i) (gatenet/net.py:112-119); the last layer has no
+    activation.  Only the wgmma back end implements it."""
     lead = x.shape[:-1]
+    if gates is not None:
+        if BACKEND != "tcgen05":
+            raise ValueError("the gated tower runs on the wgmma back end only")
+        if last_act or len(gates) != len(weights) - 1:
+            raise ValueError("gated tower: one gate per hidden layer and no last activation")
+        y = _GatedTowerTcFn.apply(x.reshape(-1, x.shape[-1]).contiguous(), len(weights), *weights,
+                                  *biases, *gates)
+        return y.reshape(*lead, y.shape[-1])
     fn = _TowerTcFn if BACKEND == "tcgen05" else _TowerFn
     y = fn.apply(x.reshape(-1, x.shape[-1]).contiguous(), len(weights), last_act, *weights, *biases)
     return y.reshape(*lead, y.shape[-1])
