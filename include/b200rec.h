@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define B200REC_ABI_VERSION 6
+#define B200REC_ABI_VERSION 7
 
 #define B200REC_OK 0
 #define B200REC_ERR_INVALID (-1)   /* bad argument (shape, alignment, NULL) */
@@ -396,6 +396,31 @@ int b200rec_tc_head_bwd_workspace_bytes(int K, size_t* bytes_host);
 int b200rec_tc_head_bwd(const void* a_planes, int64_t lda, int K, const float* w, const float* dy,
                         void* g_planes, int64_t ldg, float* dW, float* db, int64_t M,
                         void* workspace, size_t workspace_bytes, void* stream);
+/* ESMM's two width-2 heads and the CTCVR product (models/multitask/esmm/net.py:85-111) on the
+ * towers' last ReLU'd activations h_ctr, h_cvr fp32 [B,K] (contiguous, 16-byte aligned; K a multiple
+ * of 4, K <= 256), W_t [K,2], b_t [2]:
+ *   esmm_head_fwd  z_t = h_t W_t + b_t (fp32 FMAs); p1_t = 1/(1+expf(z0-z1)), p0_t = 1/(1+expf(z1-z0))
+ *                  each on its own; writes ctr_out = p_ctr [B,2], ctr_one = p1_ctr [B,1], cvr_out,
+ *                  cvr_one likewise, ctcvr_one = p1_ctr p1_cvr [B,1], ctcvr_prop = [1-ctcvr_one,
+ *                  ctcvr_one] [B,2].
+ *   esmm_head_bwd  from the gradients of the six outputs (each may be NULL: no contribution) and the
+ *                  saved p_ctr = ctr_out, p_cvr = cvr_out: Gc = g_ctcvr_prop[:,1] + g_ctcvr_one -
+ *                  g_ctcvr_prop[:,0]; G_t = g_t_out + [0, g_t_one], G_ctr1 += Gc p1_cvr, G_cvr1 +=
+ *                  Gc p1_ctr; s_t = p0_t p1_t (G_t1 - G_t0), dz_t = [-s_t, s_t].  Writes dh_t = dz_t
+ *                  W_t^T [B,K] (no ReLU mask: the tower's backward applies it), dW_t [K,2] and db_t
+ *                  [2], summed in a fixed order (no float atomics: bit-identical across runs). */
+int b200rec_esmm_head_fwd(const float* h_ctr, const float* h_cvr, int K, const float* W_ctr,
+                          const float* b_ctr, const float* W_cvr, const float* b_cvr, float* ctr_out,
+                          float* ctr_one, float* cvr_out, float* cvr_one, float* ctcvr_prop,
+                          float* ctcvr_one, int64_t B, void* stream);
+int b200rec_esmm_head_bwd_workspace_bytes(int64_t B, int K, size_t* bytes_host);
+int b200rec_esmm_head_bwd(const float* g_ctr_out, const float* g_ctr_one, const float* g_cvr_out,
+                          const float* g_cvr_one, const float* g_ctcvr_prop,
+                          const float* g_ctcvr_one, const float* p_ctr, const float* p_cvr,
+                          const float* h_ctr, const float* h_cvr, int K, const float* W_ctr,
+                          const float* W_cvr, float* dh_ctr, float* dh_cvr, float* dW_ctr,
+                          float* db_ctr, float* dW_cvr, float* db_cvr, int64_t B, void* workspace,
+                          size_t workspace_bytes, void* stream);
 /* ---- CTR head (csrc/ctr_head.cuh) ------------------------------------------ */
 /* pred = sigmoid(a + b + c) (b, c may be NULL) and its backward dlogit = dpred * p (1-p)
  * (deepfm/net.py:47: sigmoid(y_first_order + y_second_order + y_dnn)); the mean of Paddle's

@@ -64,7 +64,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     return LIB_PATH
 
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 _P = c_void_p
 _SIG = {
     "b200rec_abi_version": (c_int, []),
@@ -152,6 +152,11 @@ _SIG = {
     "b200rec_tc_linear_bwd_dw": (c_int, [_P, c_int64, _P, c_int64, _P, c_int64, c_int, c_int, _P,
                                          c_size_t, _P]),
     "b200rec_tc_head_fwd": (c_int, [_P, c_int64, c_int, _P, _P, _P, c_int64, _P]),
+    "b200rec_esmm_head_fwd": (c_int, [_P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64,
+                                      _P]),
+    "b200rec_esmm_head_bwd_workspace_bytes": (c_int, [c_int64, c_int, POINTER(c_size_t)]),
+    "b200rec_esmm_head_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, _P, _P, _P, _P,
+                                      _P, _P, _P, _P, c_int64, _P, c_size_t, _P]),
     "b200rec_tc_head_bwd_workspace_bytes": (c_int, [c_int, POINTER(c_size_t)]),
     "b200rec_tc_head_bwd": (c_int, [_P, c_int64, c_int, _P, _P, _P, c_int64, _P, _P, c_int64, _P,
                                     c_size_t, _P]),

@@ -20,6 +20,7 @@
 #include "ffm.cuh"
 #include "fat_ffm.cuh"
 #include "gate_embed.cuh"
+#include "esmm.cuh"
 
 namespace b200rec {
 
@@ -605,6 +606,48 @@ int b200rec_tc_head_bwd(const void* a_planes, int64_t lda, int K, const float* w
   if (M > 0) { NOT_NULL(a_planes); NOT_NULL(w); NOT_NULL(dy); NOT_NULL(g_planes); NOT_NULL(workspace); }
   return launch_tower_head_bwd(a_planes, lda, K, w, dy, g_planes, ldg, dW, db, M, workspace,
                                workspace_bytes, ST(stream));
+}
+
+int b200rec_esmm_head_fwd(const float* h_ctr, const float* h_cvr, int K, const float* W_ctr,
+                          const float* b_ctr, const float* W_cvr, const float* b_cvr, float* ctr_out,
+                          float* ctr_one, float* cvr_out, float* cvr_one, float* ctcvr_prop,
+                          float* ctcvr_one, int64_t B, void* stream) {
+  if (B > 0) {
+    NOT_NULL(h_ctr); NOT_NULL(h_cvr); NOT_NULL(W_ctr); NOT_NULL(b_ctr); NOT_NULL(W_cvr);
+    NOT_NULL(b_cvr); NOT_NULL(ctr_out); NOT_NULL(ctr_one); NOT_NULL(cvr_out); NOT_NULL(cvr_one);
+    NOT_NULL(ctcvr_prop); NOT_NULL(ctcvr_one);
+  }
+  return launch_esmm_head_fwd(h_ctr, h_cvr, K, W_ctr, b_ctr, W_cvr, b_cvr, ctr_out, ctr_one,
+                              cvr_out, cvr_one, ctcvr_prop, ctcvr_one, B, ST(stream));
+}
+
+int b200rec_esmm_head_bwd_workspace_bytes(int64_t B, int K, size_t* bytes_host) {
+  NOT_NULL(bytes_host);
+  B200_REQUIRE(B >= 0 && esmm_k_ok(K), "esmm_head_bwd_workspace_bytes: K=%d must be a multiple of 4 "
+               "in [4, %d]", K, kEsmmMaxK);
+  size_t bytes = 0;
+  const int rc = esmm_head_bwd_ws_bytes(B, K, &bytes);
+  if (rc != B200REC_OK) return rc;
+  *bytes_host = bytes + 16;
+  return B200REC_OK;
+}
+
+int b200rec_esmm_head_bwd(const float* g_ctr_out, const float* g_ctr_one, const float* g_cvr_out,
+                          const float* g_cvr_one, const float* g_ctcvr_prop,
+                          const float* g_ctcvr_one, const float* p_ctr, const float* p_cvr,
+                          const float* h_ctr, const float* h_cvr, int K, const float* W_ctr,
+                          const float* W_cvr, float* dh_ctr, float* dh_cvr, float* dW_ctr,
+                          float* db_ctr, float* dW_cvr, float* db_cvr, int64_t B, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  NOT_NULL(dW_ctr); NOT_NULL(db_ctr); NOT_NULL(dW_cvr); NOT_NULL(db_cvr);
+  if (B > 0) {
+    NOT_NULL(p_ctr); NOT_NULL(p_cvr); NOT_NULL(h_ctr); NOT_NULL(h_cvr); NOT_NULL(W_ctr);
+    NOT_NULL(W_cvr); NOT_NULL(dh_ctr); NOT_NULL(dh_cvr);
+  }
+  const EsmmGrads g = {g_ctr_out, g_ctr_one, g_cvr_out, g_cvr_one, g_ctcvr_prop, g_ctcvr_one};
+  return launch_esmm_head_bwd(g, p_ctr, p_cvr, h_ctr, h_cvr, K, W_ctr, W_cvr, dh_ctr, dh_cvr,
+                              dW_ctr, db_ctr, dW_cvr, db_cvr, B, workspace, workspace_bytes,
+                              ST(stream));
 }
 
 /* ---- CTR head: sigmoid of the summed logits, mean log-loss (csrc/ctr_head.cuh) --------------- */

@@ -50,6 +50,7 @@ KERNELS_PER_CALL = {
     "tc_linear_bwd_dx_db": 2, "tc_linear_bwd_dw": 2, "tc_head_fwd": 1, "tc_head_bwd": 2,
     "auc_update": 1, "sum_sigmoid_fwd": 1, "sum_sigmoid_bwd": 1, "log_loss_mean_fwd": 1, "log_loss_mean_bwd": 1, "din_attn_fwd": 2, "din_attn_bwd": 3, "gather_pool_sum": 2, "cvm_fwd": 1, "cvm_bwd": 1, "hash_keys": 1, "dot_interact_fwd": 1, "dot_interact_bwd": 1,
     "gate_embed_fwd": 1, "gate_embed_bwd": 2, "tc_gate_fwd": 1, "tc_gate_bwd": 1,
+    "esmm_head_fwd": 1, "esmm_head_bwd": 3,
 }
 # When set to a list, (name, start_event, end_event) triples are appended around the raw_* calls
 # (all of them, or only the names in EVENT_FILTER when that is a set) — bench.py's per-kernel times.
@@ -862,6 +863,64 @@ def raw_tc_gate_bwd(dz: torch.Tensor, y_planes, a: torch.Tensor):
     return g, r
 
 
+def raw_esmm_head_fwd(h_ctr: torch.Tensor, h_cvr: torch.Tensor, W_ctr: torch.Tensor,
+                      b_ctr: torch.Tensor, W_cvr: torch.Tensor, b_cvr: torch.Tensor):
+    """ESMM's two width-2 heads and the CTCVR product (multitask/esmm/net.py:85-111) from the towers'
+    last ReLU'd activations h_t [B,K]: (ctr_out [B,2], ctr_one [B,1], cvr_out [B,2], cvr_one [B,1],
+    ctcvr_prop [B,2], ctcvr_one [B,1])."""
+    lib = _lib.load()
+    h_ctr = _req(h_ctr, torch.float32, "h_ctr")
+    h_cvr = _req(h_cvr, torch.float32, "h_cvr")
+    W_ctr = _req(W_ctr.detach(), torch.float32, "W_ctr")
+    W_cvr = _req(W_cvr.detach(), torch.float32, "W_cvr")
+    b_ctr = _req(b_ctr.detach(), torch.float32, "b_ctr")
+    b_cvr = _req(b_cvr.detach(), torch.float32, "b_cvr")
+    B, K = h_ctr.shape
+    if tuple(h_cvr.shape) != (B, K) or tuple(W_ctr.shape) != (K, 2) or tuple(W_cvr.shape) != (K, 2):
+        raise _lib.B200RecError("esmm_head_fwd: h_ctr, h_cvr must be [B,K] and W_ctr, W_cvr [K,2]")
+    dev = h_ctr.device
+    two = [torch.empty(B, 2, dtype=torch.float32, device=dev) for _ in range(3)]
+    one = [torch.empty(B, 1, dtype=torch.float32, device=dev) for _ in range(3)]
+    check(lib.b200rec_esmm_head_fwd(ptr(h_ctr), ptr(h_cvr), K, ptr(W_ctr), ptr(b_ctr), ptr(W_cvr),
+                                    ptr(b_cvr), ptr(two[0]), ptr(one[0]), ptr(two[1]), ptr(one[1]),
+                                    ptr(two[2]), ptr(one[2]), B, _stream()), "esmm_head_fwd")
+    _count("esmm_head_fwd")
+    return two[0], one[0], two[1], one[1], two[2], one[2]
+
+
+def raw_esmm_head_bwd(grads, p_ctr: torch.Tensor, p_cvr: torch.Tensor, h_ctr: torch.Tensor,
+                      h_cvr: torch.Tensor, W_ctr: torch.Tensor, W_cvr: torch.Tensor):
+    """Backward of raw_esmm_head_fwd.  `grads` holds the gradients of its six outputs in order, each
+    None when that output took no gradient; p_ctr, p_cvr are the saved ctr_out, cvr_out.  Returns
+    (dh_ctr, dh_cvr, dW_ctr, db_ctr, dW_cvr, db_cvr); dh_t carries no ReLU mask."""
+    lib = _lib.load()
+    names = ("g_ctr_out", "g_ctr_one", "g_cvr_out", "g_cvr_one", "g_ctcvr_prop", "g_ctcvr_one")
+    g = [None if t is None else _req(t, torch.float32, n) for t, n in zip(grads, names)]
+    p_ctr = _req(p_ctr, torch.float32, "p_ctr")
+    p_cvr = _req(p_cvr, torch.float32, "p_cvr")
+    h_ctr = _req(h_ctr, torch.float32, "h_ctr")
+    h_cvr = _req(h_cvr, torch.float32, "h_cvr")
+    W_ctr = _req(W_ctr.detach(), torch.float32, "W_ctr")
+    W_cvr = _req(W_cvr.detach(), torch.float32, "W_cvr")
+    B, K = h_ctr.shape
+    dev = h_ctr.device
+    dh_ctr = torch.empty(B, K, dtype=torch.float32, device=dev)
+    dh_cvr = torch.empty(B, K, dtype=torch.float32, device=dev)
+    dW_ctr = torch.empty(K, 2, dtype=torch.float32, device=dev)
+    dW_cvr = torch.empty(K, 2, dtype=torch.float32, device=dev)
+    db_ctr = torch.empty(2, dtype=torch.float32, device=dev)
+    db_cvr = torch.empty(2, dtype=torch.float32, device=dev)
+    nbytes = ctypes.c_size_t(0)
+    check(lib.b200rec_esmm_head_bwd_workspace_bytes(B, K, ctypes.byref(nbytes)), "esmm_head_bwd_ws")
+    ws = workspace(nbytes.value, dev, "esmm_head")
+    check(lib.b200rec_esmm_head_bwd(*[ptr(t) for t in g], ptr(p_ctr), ptr(p_cvr), ptr(h_ctr),
+                                    ptr(h_cvr), K, ptr(W_ctr), ptr(W_cvr), ptr(dh_ctr), ptr(dh_cvr),
+                                    ptr(dW_ctr), ptr(db_ctr), ptr(dW_cvr), ptr(db_cvr), B, ptr(ws),
+                                    ws.numel(), _stream()), "esmm_head_bwd")
+    _count("esmm_head_bwd")
+    return dh_ctr, dh_cvr, dW_ctr, db_ctr, dW_cvr, db_cvr
+
+
 def _tc_bwd_ws(M: int, K: int, N: int, device, tag: str = "tc_bwd") -> torch.Tensor:
     nbytes = ctypes.c_size_t(0)
     lib = _lib.load()
@@ -1317,6 +1376,31 @@ class _GateEmbed(torch.autograd.Function):
 def gate_embed(gate_w, W, ids, dense, sink, D=None):
     """[B, F*D + Dn] gated tower input; gate_w [F] carries the autograd edge."""
     return _GateEmbed.apply(gate_w, W, ids, dense, sink, D)
+
+
+class _EsmmHead(torch.autograd.Function):
+    """ESMM's softmax heads and CTCVR product (multitask/esmm/net.py:85-111) as one kernel each way.
+    Gradients are not materialised: an output that takes no gradient reaches the kernel as NULL and
+    costs nothing."""
+
+    @staticmethod
+    def forward(ctx, h_ctr, h_cvr, W_ctr, b_ctr, W_cvr, b_cvr):
+        ctx.set_materialize_grads(False)
+        outs = raw_esmm_head_fwd(h_ctr, h_cvr, W_ctr, b_ctr, W_cvr, b_cvr)
+        ctx.save_for_backward(outs[0], outs[2], h_ctr, h_cvr, W_ctr, W_cvr)
+        return outs
+
+    @staticmethod
+    def backward(ctx, *grads):
+        p_ctr, p_cvr, h_ctr, h_cvr, W_ctr, W_cvr = ctx.saved_tensors
+        grads = [None if g is None else g.contiguous() for g in grads]
+        return raw_esmm_head_bwd(grads, p_ctr, p_cvr, h_ctr, h_cvr, W_ctr, W_cvr)
+
+
+def esmm_head(h_ctr, h_cvr, W_ctr, b_ctr, W_cvr, b_cvr):
+    """(ctr_out, ctr_one, cvr_out, cvr_one, ctcvr_prop, ctcvr_one) from the towers' last ReLU'd
+    activations h_ctr, h_cvr [B,K] and the last Linears W_t [K,2], b_t [2]."""
+    return _EsmmHead.apply(h_ctr, h_cvr, W_ctr, b_ctr, W_cvr, b_cvr)
 
 
 def gather_pool_sum(W, keys, offsets, padding_idx, sink, hook):
@@ -1812,6 +1896,6 @@ for _n in ("group_ids", "embed_fm_bwd", "ffm_fwd", "ffm_bwd", "fat_ffm_pool_fwd"
            "tc_split", "tc_split_bwd", "tc_prep_weight", "tc_linear_fwd", "tc_cross_fwd",
            "tc_linear_bwd_dx", "tc_linear_bwd_dw", "tc_head_fwd", "tc_head_bwd", "din_attn_fwd", "din_attn_bwd", "tower_split",
            "tower_relu_bwd_split", "tower_prep_weight", "tower_fold_dw", "gate_embed_fwd",
-           "gate_embed_bwd", "tc_gate_fwd", "tc_gate_bwd"):
+           "gate_embed_bwd", "tc_gate_fwd", "tc_gate_bwd", "esmm_head_fwd", "esmm_head_bwd"):
     globals()["raw_" + _n] = _wrap_timed(globals()["raw_" + _n], _n)
 del _n
